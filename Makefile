@@ -1,8 +1,8 @@
-# Builds the product library  vkfft_b200/lib/libb200fft.so  (CUDA, sm_100a only).
+# Builds the product library  vkfft_b200/lib/libb200fft.so  (CUDA, sm_90a only).
 # `make -j8`; __graft_entry__.build() calls this.  Objects go to build/ (git-ignored).
 NVCC      ?= nvcc
 CXX       ?= g++
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS   := -std=c++17 -O3 $(ARCH) -lineinfo -Xcompiler -fPIC -Ivkfft_b200/csrc -Iinclude
 CXXFLAGS  := -std=c++17 -O2 -fPIC -Ivkfft_b200/csrc -Iinclude
 SRC       := vkfft_b200/csrc

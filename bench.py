@@ -25,6 +25,7 @@
   vkfft_cuda_ref  the UNMODIFIED reference (CUDA backend, oracle/_ref) timed on the same GPU in the same run.
 
 Launch:  python bench.py --gpus 1 --steps K --warmup W          (N>1: via torch.distributed.run, one rank per GPU)
+         python bench.py ... --dump-outputs DIR                 (also writes what the last timed step computed, see dump_outputs)
          python bench.py --impl reference ...                   (the reference arm: CPU implementation of the path)
 """
 import argparse
@@ -46,6 +47,7 @@ os.environ.pop("OMP_NUM_THREADS", None)
 LOG2_MIN, LOG2_MAX = 7, 22
 TOTAL_LOG2 = 28                      # 2^28 complex64 = 2 GiB
 CPU_SAMPLE_LOG2 = 26                 # bounded sample for the CPU legs: 2^26 points (512 MiB) per N
+DUMP_POINTS = 1 << 22                # --dump-outputs: complex points sampled from the 2^28-point buffer (32 MiB as float32)
 
 
 def sizes():
@@ -64,7 +66,7 @@ def measured_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "MEASURED_PEAKS.json (driver-measured copy bandwidth)"
         except Exception:
             pass
-    return 6650.0, "fallback from B200_PROFILING.md (MEASURED_PEAKS.json absent)"
+    return 3350.0, "H100 SXM data sheet HBM3 bandwidth (MEASURED_PEAKS.json absent)"
 
 
 class ClockSampler:
@@ -455,6 +457,17 @@ def bench_dist_2p26(torch, dist, vk, local_rank, rank, world):
     return rec
 
 
+def dump_outputs(outdir, buf):
+    """What the caller of the timed path holds after its last step: the buffer every N was transformed in, forward then
+    inverse, in place.  A fixed, seeded sample of its complex64 points, as float32 (re, im) pairs, to DIR/sweep_buffer.npy."""
+    import numpy as np
+    import torch
+    os.makedirs(outdir, exist_ok=True)
+    idx = np.sort(np.random.default_rng(0).choice(buf.numel(), DUMP_POINTS, replace=False))
+    pts = torch.view_as_real(buf)[torch.from_numpy(idx).to(buf.device)].cpu().numpy()
+    np.save(os.path.join(outdir, "sweep_buffer.npy"), pts)
+
+
 # ------------------------------------------------------------------------------------------------------------------
 def run_reference_arm(args, rank, world):
     """--impl reference: the reference's CPU implementation of the path (its FFTW precision-test path; pocketfft
@@ -496,6 +509,7 @@ def main():
     ap.add_argument("--no-configs", action="store_true", help="skip the BASELINE config 3-5 legs")
     ap.add_argument("--no-sample0", action="store_true", help="skip the reference's sample_0 benchmark binaries")
     ap.add_argument("--no-dist", action="store_true", help="skip the distributed 2^26 record (N >= 2)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write a sample of the last timed step's output to DIR/*.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -564,6 +578,8 @@ def main():
     e1.record()
     barrier()
     ms_total = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, buf)
     clocks = sampler.stop() if rank == 0 else None
     ms_step = ms_total / args.steps
     if dist is not None:
@@ -622,15 +638,6 @@ def main():
                         ms_per_launch=round(ms_dom, 4), launches_per_step=e["launches"],
                         how="largest share of the step's device time; per-launch CUDA events on the launch stream "
                             "(b200fft_debug_exec_timed), mean over its launches in the sweep")
-        tr = os.path.join(ROOT, "profiles", "traffic.json")
-        if os.path.exists(tr):
-            try:
-                for rec in json.load(open(tr)):
-                    if rec["kernel"] in k or k in rec["kernel"]:
-                        roofline["traffic"] = rec["dram_bytes_per_launch"]
-                        roofline["traffic_source"] = rec.get("source")
-            except Exception:
-                pass
 
     # restore a sane buffer and verify the round trip the bench has been doing (normalize=1 -> identity)
     torch.view_as_real(buf).uniform_(-1, 1, generator=g)
@@ -730,7 +737,7 @@ def main():
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": {"workload": "configs[1]: batched 1D C2C FP32 sweep N=2^7..2^22, batch=2^28/N (2 GiB buffer per GPU), "
                                "in place, forward+inverse per N (reference sample_0 semantics, normalize=1)",
-                   "l2": "inputs (2 GiB) larger than L2 (126 MB)", "parallelism": f"batch-sharded x{world}, no collective",
+                   "l2": "inputs (2 GiB) larger than L2 (50 MB)", "parallelism": f"batch-sharded x{world}, no collective",
                    "points_per_gpu": pts},
         "roofline": roofline, "e2e": e2e, "gpu_launches": launches_per_step * args.steps * world, "clocks": clocks,
         "kernel_shares": kernel_shares, "per_n": per_n, "roundtrip_rel_err": rt_err, "numa": numa,

@@ -1,4 +1,4 @@
-/* b200fft -- C ABI of the B200-native FFT engine (libb200fft.so).
+/* b200fft -- C ABI of the H100-native FFT engine (libb200fft.so).
  *
  * This is the drop-in boundary for the reference's hot path.  The reference exposes the path as three
  * `static inline` functions in a header (everything else is reached through them):

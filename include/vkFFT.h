@@ -1,5 +1,5 @@
 /* vkFFT.h -- header-only drop-in for the CUDA backend (VKFFT_BACKEND==1) of DTolm/VkFFT, backed by the
- * B200-native engine in libb200fft.so.
+ * H100-native engine in libb200fft.so.
  *
  * User code written against the reference keeps compiling unchanged:
  *
@@ -10,7 +10,7 @@
  *     deleteVkFFT(&app);                   // reference: vkFFT_DeleteApp.h:28
  *
  * What changes underneath: no kernel text is generated; the three calls forward to the C ABI in b200fft.h (plain
- * pointers and sizes), which launches hand-written sm_100a kernels -- compiled ahead of time for the powers of two and the
+ * pointers and sizes), which launches hand-written sm_90a kernels -- compiled ahead of time for the powers of two and the
  * curated lengths, instantiated from the same templates at plan time for other smooth lengths (csrc/jit.cpp).
  * VkFFTConfiguration / VkFFTLaunchParams keep the reference's member names, order and types for
  * VKFFT_BACKEND==1 (vkFFT_Structs.h:93-379) so that sizeof/offsetof agree with the reference build
@@ -119,7 +119,7 @@ typedef struct {
     pfUINT registerBoost, registerBoostNonPow2, registerBoost4Step;
     pfUINT devicePageSize, localPageSize;
 
-    /* filled in by initializeVkFFT in the reference; reported here for the B200 the plan was made on */
+    /* filled in by initializeVkFFT in the reference; reported here for the GPU the plan was made on */
     pfUINT computeCapabilityMajor, computeCapabilityMinor;
     pfUINT maxComputeWorkGroupCount[VKFFT_MAX_FFT_DIMENSIONS];
     pfUINT maxComputeWorkGroupSize[VKFFT_MAX_FFT_DIMENSIONS];
@@ -362,7 +362,7 @@ static inline VkFFTResult initializeVkFFT(VkFFTApplication* app, VkFFTConfigurat
         if (dir) app->localFFTPlan_inverse = pl; else app->localFFTPlan = pl;
     }
     if (c->saveApplicationToString) {   /* the plan holds no generated binary worth saving, so the "binary" is a tag */
-        static const char tag[] = "b200fft:aot:sm_100a";
+        static const char tag[] = "b200fft:aot:sm_90a";
         app->saveApplicationString = malloc(sizeof tag);
         if (!app->saveApplicationString) { deleteVkFFT(app); return VKFFT_ERROR_MALLOC_FAILED; }
         memcpy(app->saveApplicationString, tag, sizeof tag);

@@ -12,7 +12,7 @@ sample_16_...dct.cpp:138-198).  FFTW is not installed in this image, so the same
 evaluated with pocketfft (scipy.fft); `dft_definition` below is the literal O(N^2) sum used to pin pocketfft,
 and oracle/stockham_ref.c restates the reference's Stockham/Four-Step algorithm itself.
 Pinning: tests/test_oracle.py checks all of these against each other and against tests/golden/*.npz, which
-hold outputs of the reference's CUDA backend (generated on a B200 by tests/golden/make_golden.py).
+hold outputs of the reference's CUDA backend (generated on a GPU by tests/golden/make_golden.py).
 """
 import ctypes
 import os

@@ -10,7 +10,7 @@ for p in (ROOT, os.path.join(ROOT, "tests"), os.path.join(ROOT, "tests", "emu"),
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an NVIDIA H100 (select with -m gpu)")
 
 
 @pytest.fixture(scope="session")

@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE ONLY -- never linked into the product library.
 //
 // A tiny CPU emulation of the CUDA execution model, good enough to run the engine's kernel *bodies*
-// (the same templates nvcc compiles for sm_100a) inside the CPU test-suite: one OS thread per CUDA
+// (the same templates nvcc compiles for sm_90a) inside the CPU test-suite: one OS thread per CUDA
 // thread of a block, a std::barrier for __syncthreads(), blocks executed one after another.
 // It exists because the development container has no GPU: index maps, twiddle tables and the autosort
 // scatter are checked here against the double-precision oracle before GPU minutes are spent, and the
@@ -136,7 +136,7 @@ inline ConflictReport analyse(unsigned nthreads) {
 template <class F>
 inline void launch(unsigned grid, unsigned block, size_t smem_bytes, F&& f, bool log = false) {
     State& s = st();
-    // what cudaLaunchKernel would refuse on sm_100 (1024 threads, 227 KiB opt-in shared memory, 2^31-1 CTAs)
+    // what cudaLaunchKernel would refuse on sm_90 (1024 threads, 227 KiB opt-in shared memory, 2^31-1 CTAs)
     if (block == 0 || block > 1024 || smem_bytes > 232448 || grid == 0 || grid > 0x7fffffffu) { s.launch_refused = true; return; }
     s.blockDim = {block, 1, 1};
     s.gridDim = {grid, 1, 1};

@@ -1,6 +1,7 @@
 """CPU: the C-ABI library loads, exports every symbol include/b200fft.h declares, the header-only vkFFT.h shim
 compiles as C and C++ with the reference's struct layout, and host-side error behaviour matches the reference.
 (No compute calls here: there is no GPU in the -m "not gpu" environment.)"""
+import json
 import os
 import re
 import subprocess
@@ -92,8 +93,8 @@ def _layout_dump(include_dirs, defines, members, lang):
 def test_vkfft_shim_header_layout(lang):
     """sizeof/offsetof of the drop-in structs == the reference's VKFFT_BACKEND==1 build.  The probe is compiled, RUN and
     compared: against the known numbers of the reference headers (SURVEY.md section 7: VkFFTConfiguration 1168 B,
-    VkFFTLaunchParams 80 B, buffer@152, numberBatches@272, doublePrecision@360, performR2C@408) and -- when the reference
-    tree is present -- member by member against a probe compiled from the reference's own header."""
+    VkFFTLaunchParams 80 B, buffer@152, numberBatches@272, doublePrecision@360, performR2C@408) and member by member
+    against the same probe compiled from the reference's own header (stored in tests/golden)."""
     cuda = "/usr/local/cuda"
     if not os.path.exists(os.path.join(cuda, "include", "cuda.h")):
         pytest.skip("CUDA headers not present")
@@ -105,10 +106,10 @@ def test_vkfft_shim_header_layout(lang):
     assert mine["sizeof.VkFFTConfiguration"] == 1168 and mine["sizeof.VkFFTLaunchParams"] == 80
     assert mine["VkFFTConfiguration.buffer"] == 152 and mine["VkFFTConfiguration.numberBatches"] == 272
     assert mine["VkFFTConfiguration.doublePrecision"] == 360 and mine["VkFFTConfiguration.performR2C"] == 408
-    ref_inc = "/root/reference/vkFFT"
-    if lang == "c++" and os.path.exists(os.path.join(ref_inc, "vkFFT.h")):
-        theirs = _layout_dump([ref_inc], ["VKFFT_BACKEND=1"], members, lang)
-        assert mine == theirs, {k: (mine[k], theirs.get(k)) for k in mine if mine[k] != theirs.get(k)}
+    # the same probe compiled (as C++) against the reference's vkFFT.h 1.3.4, stored as tests/golden/vkfft_struct_layout.json
+    with open(os.path.join(ROOT, "tests", "golden", "vkfft_struct_layout.json")) as f:
+        theirs = json.load(f)
+    assert mine == theirs, {k: (mine.get(k), theirs.get(k)) for k in set(mine) | set(theirs) if mine.get(k) != theirs.get(k)}
 
 
 def test_python_api_host_side_errors(built_lib):
@@ -150,19 +151,3 @@ def test_reference_style_cpp_program_runs(built_lib):
     with tempfile.TemporaryDirectory() as td:
         out = subprocess.run([_build_sample(td)], capture_output=True, text=True)
         assert out.returncode == 0, out.stdout + out.stderr
-
-
-def test_reference_testsuite_sources_build_against_the_shim(built_lib):
-    """drop-in at source level: the reference's own VkFFT_TestSuite.cpp with its benchmark / convolution samples and utilities
-    (unmodified, where they lie) compiles against include/vkFFT.h and links to libb200fft.so"""
-    if not os.path.isdir("/root/reference/benchmark_scripts"):
-        pytest.skip("reference tree not present")
-    exe = os.path.join(ROOT, "oracle", "_ref", "VkFFT_TestSuite_b200")
-    if os.path.exists(exe):
-        os.unlink(exe)
-    subprocess.check_call(["make", "-C", os.path.join(ROOT, "oracle"), "testsuite"], stdout=subprocess.DEVNULL)
-    assert os.path.exists(exe)
-    syms = subprocess.run(["nm", "-D", "--undefined-only", exe], capture_output=True, text=True).stdout
-    for s in ("b200fft_plan_create", "b200fft_exec", "b200fft_plan_destroy", "b200fft_plan_axis_uploads"):
-        assert s in syms, s                      # the samples' initializeVkFFT / VkFFTAppend / deleteVkFFT end in the C ABI
-    assert "nvrtcCompileProgram" not in syms     # nothing is JIT-compiled any more

@@ -1,4 +1,4 @@
-"""CPU: the kernel *bodies* (the same templates nvcc compiles for sm_100a) run on the thread-per-CUDA-thread
+"""CPU: the kernel *bodies* (the same templates nvcc compiles for sm_90a) run on the thread-per-CUDA-thread
 emulation in tests/emu and are compared with the oracle; whole plans (planner + kernels) too.  This is how
 index maps, twiddle tables, the autosort scatter and the Four-Step plumbing are verified without a GPU."""
 import os

@@ -1,4 +1,4 @@
-"""CPU: thinned versions of the exhaustive emulation sweeps of profiles/r1/emu_sweeps.md (the reference's precision samples
+"""CPU: thinned versions of the exhaustive emulation sweeps of tools/emu_sweep_*.py (the reference's precision samples
 11-18 walk size ranges the same way: sample_11/14/15/16_precision_VkFFT_*.cpp)."""
 import os
 import sys

@@ -37,7 +37,7 @@ def test_bluestein_c2c(shape, b, prec, inv):
 @pytest.mark.parametrize("shape,b,prec", [((77,), 5, 0), ((1430,), 2, 0), ((2 * 3 * 5 * 7 * 11,), 1, 1), ((66, 26), 2, 0), ((13,), 9, 0)])
 @pytest.mark.parametrize("inv", [-1, 1])
 def test_runtime_scheduled_kernel_first_and_last_stage_from_registers(shape, b, prec, inv, monkeypatch):
-    """generic.cuh::stage_io (opt-in, B200FFT_GENERIC_FUSED_IO=1: measured slower than the separate copy phases on B200, kept
+    """generic.cuh::stage_io (opt-in, B200FFT_GENERIC_FUSED_IO=1: measured slower than the separate copy phases, kept
     for the record): the first butterflies read the lines from global memory, the last ones write them, operators in registers"""
     monkeypatch.setenv("B200FFT_GENERIC_FUSED_IO", "1")
     dt = np.complex64 if prec == 0 else np.complex128
@@ -106,7 +106,7 @@ def test_bluestein_one_launch_equals_two_launches(monkeypatch):
 def test_rader_prime_radix_stages(shape, b, prec, inv, monkeypatch):
     """prime factors 17..127 as Rader stages inside one shared-memory pass (reference probe: 1088 = 17.16.4,
     2032 = 8.127.2, 12167 = 23^3 in two passes; SURVEY.md appendix C).  Since the GPU timings of round 2 the planner only
-    takes this path above 2048 points (below, Bluestein is faster: profiles/r2/rader_vs_bluestein.log); the switch keeps
+    takes this path above 2048 points (below, Bluestein is faster); the switch keeps
     the Rader code under test at every length."""
     monkeypatch.setenv("B200FFT_RADER_MAX_PRIME", "127")
     dt = np.complex64 if prec == 0 else np.complex128

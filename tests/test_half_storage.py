@@ -201,11 +201,9 @@ def test_c2c_half_storage_vs_oracle(gpu, shape, batch, inverse):
 
 @pytest.mark.gpu
 def test_half_storage_timing_is_reported(gpu):
-    """2^27 points, N = 4096.  Measured on B200: FP32 storage 0.330 ms (the copy roofline), half storage 0.375 ms -- the
-    single-pass kernels are bound by load/store ISSUE, not by bytes (ncu: LSU wavefronts 70-80 %), and the half variant issues
-    the same number of (32-bit instead of 64-bit) accesses plus the conversions, so halving the bytes does not halve the time;
-    the Four-Step sizes, whose strided passes are byte-bound, do gain (sample_2: 2^19 1.52 ms vs 2.00 for the reference).  The
-    test records the two numbers and only guards against a pathological kernel."""
+    """2^27 points, N = 4096.  The half variant issues the same number of (32-bit instead of 64-bit) accesses plus the
+    conversions, so halving the bytes need not halve the time of a single-pass kernel.  The test records the two numbers
+    and only guards against a pathological kernel."""
     import torch
     import vkfft_b200 as vk
     n, batch = 4096, 1 << 15

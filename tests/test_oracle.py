@@ -75,7 +75,7 @@ def test_real_transform_definitions():
 
 
 def test_golden_vectors_from_reference_cuda_backend():
-    """tests/golden/*.npz were produced by the reference itself (CUDA backend) on a B200; the oracle must agree
+    """tests/golden/*.npz were produced by the reference itself (CUDA backend); the oracle must agree
     with them to the reference's own single/double precision accuracy."""
     files = sorted(glob.glob(os.path.join(GOLD, "*.npz")))
     if not files:

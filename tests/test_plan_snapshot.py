@@ -1,5 +1,6 @@
-"""CPU: the planner's choices for the headline workload are the measured-best ones (profiles/r2/ktune_f32.log: every
-registered kernel timed alone on a 2 GiB pass after the packed-FP32 rewrite).  A change here is a performance change: re-measure with tools/ktune.py / bench.py before updating."""
+"""CPU: the planner's choices for the headline workload are the measured-best ones (the pass costs in
+planner.cpp::split_four_step: every registered kernel timed alone on a 2 GiB pass by tools/ktune.py).  A change here is a
+performance change: re-measure with tools/ktune.py / bench.py before updating."""
 import os
 import re
 import sys
@@ -13,9 +14,9 @@ SWEEP = {
     7: [("128", "ROWS")], 8: [("256", "ROWS")], 9: [("512", "ROWS")], 10: [("1024", "ROWS")], 11: [("2048", "ROWS")],
     12: [("4096", "ROWS")], 13: [("8192", "ROWS")], 14: [("16384", "PIPE1_ROWS")],
     15: [("128", "COLS"), ("256", "ROWS_TOUT")], 16: [("128", "COLS"), ("512", "ROWS_TOUT")],
-    17: [("128", "COLS"), ("1024", "ROWS_TOUT")], 18: [("256", "COLS"), ("1024", "ROWS_TOUT")],
-    19: [("512", "COLS"), ("1024", "ROWS_TOUT")], 20: [("1024", "COLS"), ("1024", "ROWS_TOUT")],
-    21: [("1024", "COLS"), ("2048", "PIPE1_ROWS_TOUT")], 22: [("128", "COLS"), ("128", "COLS"), ("256", "ROWS_TOUT")],
+    17: [("128", "COLS"), ("1024", "ROWS_TOUT")], 18: [("512", "COLS"), ("512", "ROWS_TOUT")],
+    19: [("512", "COLS"), ("1024", "ROWS_TOUT")], 20: [("2048", "COLS"), ("512", "ROWS_TOUT")],
+    21: [("2048", "COLS"), ("1024", "ROWS_TOUT")], 22: [("128", "COLS"), ("128", "COLS"), ("256", "ROWS_TOUT")],
 }
 
 

@@ -1,4 +1,4 @@
-"""Bug hunt on the CPU emulation of the kernels (no GPU): see profiles/r1/emu_sweeps.md for the runs of round 1."""
+"""Bug hunt on the CPU emulation of the kernels (no GPU)."""
 import os, sys, time, json
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'tests', 'emu')); 
 import numpy as np, emu, scipy.fft as sfft

@@ -1,7 +1,7 @@
 // Complex arithmetic + host/device portability macros shared by every kernel in the engine.
 //
 // The same headers are compiled three ways:
-//   * nvcc for sm_100a            -> the product (libb200fft.so)
+//   * nvcc for sm_90a             -> the product (libb200fft.so)
 //   * g++ with tests/emu/cuda_emu.h -> a CPU "one OS thread per CUDA thread" emulation used only by
 //                                    the CPU test-suite to check index maps / bank conflicts
 //   * g++ for the host planner (only the POD parts)
@@ -71,66 +71,45 @@ inline void b2_h2_to_f2(uint32_t h, float& re, float& im) { re = b2_half_bits_to
 inline uint32_t b2_f2_to_h2(float re, float im) { return (uint32_t)b2_float_to_half_bits(re) | ((uint32_t)b2_float_to_half_bits(im) << 16); }
 #endif
 
-// FP32 complex arithmetic on sm_100a uses the packed two-lane instructions (FADD2 / FMUL2 / FFMA2, PTX add/mul/fma.f32x2):
-// one instruction per complex add, two per complex multiply, and quarter turns / conjugation are operand modifiers
-// (the SASS operands take a .LO_HI swap, a per-half negation and a 32-bit broadcast), so an interleaved (re, im) pair
-// is processed whole.  These kernels are issue-bound (profiles/README.md), and this halves their floating-point
-// instruction count.  The reference emits scalar code for every backend (vkFFT_MathUtils.h).  Host code, the CPU
-// emulation and FP64 use the plain component-wise form below; results agree to rounding (same operations, the product
-// a.x*b.x is rounded before the fused multiply-add instead of a.y*b.y).
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ >= 1000) && !defined(B2_NO_F32X2)
-#define B2_F32X2 1
-#define B2_PK(a) make_float2((a).x, (a).y)
-template <typename T> B2_D cpx<T> b2_unpk(float2 v) { return mk<T>((T)v.x, (T)v.y); }
-#else
-#define B2_F32X2 0
-#endif
-
+// FP32 complex arithmetic on the device is spelled out with the round-to-nearest intrinsics, which the compiler never
+// contracts or reorders: every kernel that runs the same stage code -- a stand-alone pass or the same pass inside the
+// fused Four-Step launch -- then rounds identically, whatever code surrounds it.  The product rounds a.x*b.x (a.y*b.x)
+// before the fused multiply-add.  Host code, the CPU emulation and FP64 use the plain component-wise form.
 template <typename T> B2_HD cpx<T> operator+(cpx<T> a, cpx<T> b) {
-#if B2_F32X2
-    if constexpr (sizeof(T) == 4) return b2_unpk<T>(__fadd2_rn(B2_PK(a), B2_PK(b)));
-    else
+#if defined(__CUDA_ARCH__)
+    if constexpr (sizeof(T) == 4) return mk<T>(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y));
 #endif
     return mk<T>(a.x + b.x, a.y + b.y);
 }
 template <typename T> B2_HD cpx<T> operator-(cpx<T> a, cpx<T> b) {
-#if B2_F32X2
-    if constexpr (sizeof(T) == 4) return b2_unpk<T>(__fadd2_rn(B2_PK(a), make_float2(-b.x, -b.y)));
-    else
+#if defined(__CUDA_ARCH__)
+    if constexpr (sizeof(T) == 4) return mk<T>(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y));
 #endif
     return mk<T>(a.x - b.x, a.y - b.y);
 }
 template <typename T> B2_HD cpx<T> operator*(cpx<T> a, cpx<T> b) {
-#if B2_F32X2
-    if constexpr (sizeof(T) == 4) {
-        const float2 p = __fmul2_rn(B2_PK(a), make_float2(b.x, b.x));
-        return b2_unpk<T>(__ffma2_rn(make_float2(-a.y, a.x), make_float2(b.y, b.y), p));
-    } else
+#if defined(__CUDA_ARCH__)
+    if constexpr (sizeof(T) == 4) return mk<T>(__fmaf_rn(-a.y, b.y, __fmul_rn(a.x, b.x)), __fmaf_rn(a.x, b.y, __fmul_rn(a.y, b.x)));
 #endif
     return mk<T>(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x);
 }
 template <typename T> B2_HD cpx<T> operator*(cpx<T> a, T s) {
-#if B2_F32X2
-    if constexpr (sizeof(T) == 4) return b2_unpk<T>(__fmul2_rn(B2_PK(a), make_float2(s, s)));
-    else
+#if defined(__CUDA_ARCH__)
+    if constexpr (sizeof(T) == 4) return mk<T>(__fmul_rn(a.x, s), __fmul_rn(a.y, s));
 #endif
     return mk<T>(a.x * s, a.y * s);
 }
 // a * conj(b)
 template <typename T> B2_HD cpx<T> mulc(cpx<T> a, cpx<T> b) {
-#if B2_F32X2
-    if constexpr (sizeof(T) == 4) {
-        const float2 p = __fmul2_rn(B2_PK(a), make_float2(b.x, b.x));
-        return b2_unpk<T>(__ffma2_rn(make_float2(a.y, -a.x), make_float2(b.y, b.y), p));
-    } else
+#if defined(__CUDA_ARCH__)
+    if constexpr (sizeof(T) == 4) return mk<T>(__fmaf_rn(a.y, b.y, __fmul_rn(a.x, b.x)), __fmaf_rn(-a.x, b.y, __fmul_rn(a.y, b.x)));
 #endif
     return mk<T>(a.x * b.x + a.y * b.y, a.y * b.x - a.x * b.y);
 }
 // c + a * s  (real scalar s)
 template <typename T> B2_HD cpx<T> fma_s(cpx<T> a, T s, cpx<T> c) {
-#if B2_F32X2
-    if constexpr (sizeof(T) == 4) return b2_unpk<T>(__ffma2_rn(B2_PK(a), make_float2(s, s), B2_PK(c)));
-    else
+#if defined(__CUDA_ARCH__)
+    if constexpr (sizeof(T) == 4) return mk<T>(__fmaf_rn(a.x, s, c.x), __fmaf_rn(a.y, s, c.y));
 #endif
     return mk<T>(c.x + a.x * s, c.y + a.y * s);
 }

@@ -3,7 +3,7 @@
 // The reference (and this engine's two-launch plan) writes the whole intermediate to DRAM in the first dispatch and
 // reads it back in the second (vkFFT_Scheduler.h:2582-2893: "numAxisUploads = 2"), i.e. two HBM round trips, which caps
 // those sizes at 0.5 of the copy roofline.  Here:
-//   * sequences are grouped into UNITS; the scratch is a ring of R units (a few MB ... tens of MB, far below the 126 MB
+//   * sequences are grouped into UNITS; the scratch is a ring of R units (a few MB ... tens of MB, below the H100's 50 MB
 //     L2), rewritten over and over, so it lives in L2: pass A's stores and pass B's loads never reach HBM;
 //   * persistent CTAs take TILES from two ordered queues.  A tile of pass A (Q_A neighbouring columns of one sequence:
 //     strided n1-point transforms + the Four-Step phase) may be taken when its unit's ring slot is free; a tile of pass B
@@ -118,7 +118,7 @@ struct Fused4 {
     // together is 2 * NG sequences (tens of MB at most: K is chosen by the planner so that it stays far below the L2 size)
     // and is rewritten in place for the whole launch, so it never leaves L2.  (Three dynamic schedulers -- semaphores,
     // reserved tickets, one ordered queue -- were measured first: every ticket a CTA holds ahead of its work widens the
-    // window of units that must stay resident and the CTAs ended up waiting for each other, profiles/r2/fused_*.log.)
+    // window of units that must stay resident and the CTAs ended up waiting for each other.)
     // The counter updates of a tile (one MEMBAR.GPU + one atomic) and the refresh of the two counters are issued behind the
     // NEXT tile's first butterflies and only looked at after its last store: no memory round trip on the tile path.
     struct Sched {
@@ -211,7 +211,7 @@ struct Fused4 {
         if (c.kind == TILE_A) {
 #if defined(__CUDA_ARCH__)
             // one tensor copy per box of up to 256 rows: the TMA unit walks the rows (row-by-row bulk copies cost ~50 cycles
-            // of the unit each and made the launch several times slower, profiles/r2/fused_exp_bulk_rows.log)
+            // of the unit each and made the launch several times slower)
             if (lane == 0) {
                 mbar_expect_tx(bar, BYTES_A);
 #pragma unroll

@@ -2,8 +2,7 @@
 //
 // The ahead-of-time registry (kernel_list*.def) covers the powers of two, ~230 curated lengths and every Four-Step factor
 // the BASELINE configurations need.  Any other 2..31-smooth length used to fall back to the runtime-scheduled kernel
-// (generic.cuh), which is 3-5x slower than a specialised one (profiles/r2/bluestein_one_launch_vs_two.log: N = 1100
-// 1.33 ms against 0.35 ms for the reference).  Here such a length gets `Engine<KCfg<...>>` of stockham.cuh -- the very code
+// (generic.cuh), which is several times slower than a specialised one.  Here such a length gets `Engine<KCfg<...>>` of stockham.cuh -- the very code
 // of the ahead-of-time kernels, with its own radix schedule and CTA shape as template constants -- compiled for the
 // device's architecture when the plan that needs it is created: NVRTC -> cubin -> cuModuleLoadData.  ~2 s per length, once
 // per process.  The reference compiles EVERY kernel of EVERY plan like that (vkFFT_CompileKernel.h:299-491: NVRTC,
@@ -269,7 +268,7 @@ std::string cache_path(const Program& p, const char* arch, bool lineinfo) {
     return std::string(dir) + name;
 }
 
-// NVRTC -> cubin for `arch` ("sm_100a"); no GPU needed
+// NVRTC -> cubin for `arch` ("sm_90a"); no GPU needed
 int compile(Program& p, const char* arch) {
     Api& a = api();
     const bool lineinfo = getenv("B200FFT_JIT_LINEINFO") != nullptr;
@@ -373,7 +372,7 @@ extern "C" int b2_jit_prepare(const b2_kernel_info* k) {
     if (a.CtxGetDevice(&dev) != 0) return -1;
     Program& p = *e->prog;
     if (p.compiled == 0) {
-        int major = 10, minor = 0;
+        int major = 9, minor = 0;
         a.DeviceGetAttribute(&major, 75 /* CU_DEVICE_ATTRIBUTE_COMPUTE_CAPABILITY_MAJOR */, dev);
         a.DeviceGetAttribute(&minor, 76 /* ..._MINOR */, dev);
         char arch[32];
@@ -419,7 +418,7 @@ extern "C" int b2_jit_launch(const b2_kernel_info* k, const b2_pass_params* P, u
     return a.LaunchKernel(fn, grid, 1, 1, (unsigned)k->threads, 1, 1, (unsigned)e->shape.smem, (CUstream)stream, args, nullptr);
 }
 
-// CPU-side self test (no GPU): describe + compile the kernel for (kind, prec, n, ops) to a cubin for sm_100a.
+// CPU-side self test (no GPU): describe + compile the kernel for (kind, prec, n, ops) to a cubin for sm_90a.
 // Returns the cubin size, 0 if the key is not eligible, < 0 on a compile error (log through b2_jit_last_log).
 extern "C" long b2_jit_selftest(int kind, int prec, int n, int ops) {
     const b2_kernel_info* k = provide(kind, prec, n, 0, ops);
@@ -427,7 +426,7 @@ extern "C" long b2_jit_selftest(int kind, int prec, int n, int ops) {
     Entry* e = (Entry*)k->jit;
     std::lock_guard<std::mutex> lk(g_mu);
     Program& p = *e->prog;
-    if (p.compiled == 0) p.compiled = compile(p, "sm_100a") == 0 ? 1 : -1;
+    if (p.compiled == 0) p.compiled = compile(p, "sm_90a") == 0 ? 1 : -1;
     if (p.compiled < 0) { g_last_log = p.log; return -1; }
     return (long)p.cubin.size();
 }

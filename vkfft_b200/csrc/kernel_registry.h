@@ -1,6 +1,6 @@
 // Registry of kernel instantiations.  The planner looks kernels up by (kind, precision, length, direction, fused-operator
 // set).  The hot path -- powers of two, the curated lengths, every Four-Step factor of the BASELINE configurations -- is
-// compiled ahead of time for sm_100a.  A length that is 2..31-smooth but not in the ahead-of-time lists gets the SAME
+// compiled ahead of time for sm_90a.  A length that is 2..31-smooth but not in the ahead-of-time lists gets the SAME
 // hand-written templates (stockham.cuh) instantiated for it when its plan is created (jit.cpp, NVRTC -> cubin; the product
 // library only) instead of falling back to the runtime-scheduled kernel, which is 3-5x slower.  The reference compiles every
 // kernel of every plan that way (vkFFT_CompileKernel.h:299-491); here it is the exception, and B200FFT_NO_JIT=1 turns it off.

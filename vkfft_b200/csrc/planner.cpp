@@ -274,9 +274,8 @@ int emit(PlanGraph& g, std::vector<PassPlan>& list, const PassReq& rq) {
         P.load_io = rq.load_io; P.store_io = rq.store_io;
         if (generic && getenv("B200FFT_GENERIC_FUSED_IO")) {
             // plain complex lines: the first butterflies read HBM and the last ones write it (generic.cuh stage_io) instead of
-            // separate copy phases through shared memory.  Measured on B200 and REJECTED as the default
-            // (profiles/r2/other_lengths_plan_time_templates_ab.log: N = 154 2.34 vs 2.03 ms, 4004 2.87 vs 2.29, 1100 1.60 vs 1.56 --
-            // the strided first-stage legs of a runtime radix cost more than the two shared-memory passes they save); opt-in
+            // separate copy phases through shared memory.  Measured slower and REJECTED as the default (the strided
+            // first-stage legs of a runtime radix cost more than the two shared-memory passes they save); opt-in
             if ((rq.load_io == B2_IO_C2C || rq.load_io == B2_IO_R2C_EVEN) && radices.front() <= 16) P.gen_flags |= B2_GEN_FUSE_IN;
             if ((rq.store_io == B2_IO_C2C || rq.store_io == B2_IO_C2R_EVEN) && radices.back() <= 16) P.gen_flags |= B2_GEN_FUSE_OUT;
         }
@@ -317,10 +316,9 @@ bool single_ok(const PlanGraph& g, int kind, uint64_t n, int ops) {
     return generic_fits(g, n);
 }
 
-// Fused Four-Step (fused4.cuh).  Measured on B200 (profiles/r2): DRAM traffic is exactly one read + one write (the ring stays
-// in L2), but each SM now has to turn every tile over twice in the time HBM delivers it once, and with the loads of a tile
-// on its critical path the resident CTAs do not keep enough bytes in flight: 1.56 ms (2^16) / 1.83 ms (2^20) per 2 GiB
-// transform against 1.28 / 1.67 ms for the two launches.  Opt-in (B200FFT_FUSED4=1) until the asynchronous tile prefetch is in.
+// Fused Four-Step (fused4.cuh).  DRAM traffic is exactly one read + one write (the ring stays in L2), but each SM now has to
+// turn every tile over twice in the time HBM delivers it once, and with the loads of a tile on its critical path the
+// resident CTAs do not keep enough bytes in flight: it measured slower than the two launches.  Opt-in (B200FFT_FUSED4=1).
 bool fused4_enabled() {
     const char* e = getenv("B200FFT_FUSED4");        // read per plan: tests and tuning scripts switch it between plans
     return e && *e && *e != '0' && !getenv("B200FFT_NO_FUSED4");
@@ -350,20 +348,21 @@ std::vector<uint64_t> split_four_step(const PlanGraph& g, uint64_t N, bool dist 
     }
     const uint64_t cap = std::min<uint64_t>(max_single_env(), half_plan(g) ? 512 : 4096);   // (half storage: factors up to 512 keep 16+ lines = 64-byte runs per tile of the strided / transposed side)
     auto fast = [&](int kind, uint64_t n, int ops) { return b2_find_kernel(kind, g.prec, (int)n, 0, ops) != nullptr; };
-    // measured cost of one full pass over a 2 GiB FP32 buffer on B200, microseconds (profiles/r2/ktune_f32.log);
-    // used to rank factorizations.  Unknown sizes / FP64 fall back to "balanced factors".
+    // measured cost of one full pass over a 2 GiB FP32 buffer, microseconds (tools/ktune.py, default variant of each kernel;
+    // H100 80GB HBM3 SXM at a 400 W power limit); used to rank factorizations.  Unknown sizes / FP64 fall back to
+    // "balanced factors".
     auto pass_us = [&](int kind, uint64_t n) -> uint64_t {
         if (g.prec != B2_PREC_F32) return 0;
-        static const struct { uint64_t n; uint64_t cols, tout; } t[] = {      // profiles/r2/ktune_f32.log
-            {16, 626, 1032}, {32, 627, 631}, {64, 635, 638}, {128, 635, 641}, {256, 685, 631},
-            {512, 775, 650}, {1024, 864, 685}, {2048, 1258, 900}};
+        static const struct { uint64_t n; uint64_t cols, tout; } t[] = {
+            {16, 1434, 1491}, {32, 2220, 1465}, {64, 1439, 1456}, {128, 1431, 1454}, {256, 1472, 1448},
+            {512, 1471, 1460}, {1024, 2507, 1468}, {2048, 1660, 2373}};
         for (const auto& e : t)
             if (e.n == n) return kind == B2_KIND_COLS ? e.cols : e.tout;
         return 0;
     };
     // distributed plans: the first launch's stores and the last launch's transposed stores cross NVLink in runs of
-    // q elements; 64-byte runs (q = 8) reached 430 GB/s per direction, 128-byte runs 670 GB/s (2 x B200,
-    // profiles/r1/dist_fused_split_experiment_2gpu.log) -> rank kernels with q < 16 as if their pass were 300 us slower
+    // q elements; 64-byte runs (q = 8) reach markedly less bandwidth per direction than 128-byte runs -> rank kernels with
+    // q < 16 as if their pass were 300 us slower
     auto short_runs = [&](int kind, uint64_t n, int ops) -> uint64_t {
         if (!dist) return 0;
         const b2_kernel_info* k = b2_find_kernel(kind, g.prec, (int)n, 0, ops);
@@ -397,8 +396,7 @@ std::vector<uint64_t> split_four_step(const PlanGraph& g, uint64_t N, bool dist 
         }
         if (cost < best_cost) { best_cost = cost; best = {n1, n2}; }
     }
-    // three launches of fast 128/256-point factors beat two launches with a 2048-point strided pass from 2^22 on (FP32, B200:
-    // 635 + 635 + 631 us against 1258 + 900 us per 2 GiB pass, profiles/r2/ktune_f32.log)
+    // from 2^22 on, three launches of fast 128/256-point factors (a 4096-point factor has no fast strided kernel)
     const uint64_t two_level_limit = 1ull << 21;
     if (!best.empty() && N <= two_level_limit) return best;
     std::vector<uint64_t> best3;
@@ -513,10 +511,8 @@ uint64_t count_lines(const std::vector<Dim>& lines) {
 // smallest padded length >= 2N-1 with a one-launch Bluestein kernel (stockham.cuh RMODE 11), 0 if there is none
 uint64_t blue1_length(const PlanGraph& g, uint64_t N) {
     if (getenv("B200FFT_NO_FUSED_BLUESTEIN")) return 0;
-    // measured on B200 (profiles/r2/bluestein_one_launch_vs_two.log, ms per pair of ~512 MiB): one launch wins up to a padded
-    // length of 3584 in FP32 (N = 113: 0.95 vs 1.80, 509: 1.08 vs 1.45, 1019: 1.17 vs 1.56, 1517: 1.72 vs 1.87) and ties or loses
-    // above (N = 2039, M = 4096: 1.43 vs 1.40; 4093, M = 8192: 2.24 vs 1.87 -- 32 points per thread at 2 CTAs per SM); in
-    // FP64 it wins at every length it exists for (2039: 1.79 vs 2.50)
+    // measured against the two-launch Bluestein transform: one launch wins up to a padded length of 3584 in FP32 and ties
+    // or loses above (32 points per thread at 2 CTAs per SM); in FP64 it wins at every length it exists for
     const uint64_t limit = getenv("B200FFT_FORCE_BLUESTEIN") ? ~0ull : (g.prec == B2_PREC_F32 ? 3584 : 4096);
     if (2 * N - 1 > limit) return 0;
     uint64_t M1 = 0;
@@ -706,11 +702,12 @@ void try_fuse(PlanGraph& g, std::vector<PassPlan>& list, size_t ia) {
     const uint64_t N = (uint64_t)a.P.n * b.P.n, esz = esize(g), seq_bytes = N * esz;
     // K = CTAs per group: every CTA of a group takes tiles r, r+K, ... of both passes of one sequence per phase.  One or two
     // tiles of each pass per CTA and phase keep the groups small enough to fill the device evenly and large enough that the
-    // scratch of all groups (2 sequences each) stays well inside L2:  K = max(TA, TB) / 2, at least 8, at most 148.
+    // scratch of all groups (2 sequences each) stays well inside L2:  K = max(TA, TB) / 2, at least 8, at most 132 (the
+    // H100's SMs: the CTAs of a group wait for each other, so one group must be resident at once even at one CTA per SM).
     const uint64_t ga = (a.P.G + fk->qa - 1) / fk->qa, gb = (b.P.G + fk->qb - 1) / fk->qb;
     uint64_t K = std::max<uint64_t>(std::max(ga, gb) / 2, 8);
     if (seq_bytes >= (4ull << 20)) K = std::max(ga, gb);              // long sequences: one tile per CTA and phase, fewer groups
-    K = std::min<uint64_t>(K, 148);
+    K = std::min<uint64_t>(K, 132);
     if (const char* e = getenv("B200FFT_FUSED_GROUP")) K = std::max<uint64_t>(1, strtoull(e, nullptr, 10));
     const uint64_t U = K, NU = 0, R = 2, L = 0;
     if (nseq * (ga + gb) > 0x7fffffffull) return;
@@ -755,18 +752,16 @@ int plan_c2c(PlanGraph& g, std::vector<PassPlan>& list, const C2CJob& job) {
     const bool dist = job.world > 1;
     if (dist && (!contiguous || job.unit_lines || count_lines(job.lines) != 1 || !is_smooth(N))) return R_UNSUPPORTED_FFT_LENGTH;
     if (!is_smooth(N)) return plan_bluestein(g, list, job);
-    // Measured on B200 (profiles/r2/rader_vs_bluestein.log, ~512 MiB per pair): the Rader stage of the runtime-scheduled kernel is
-    // a direct O(p^2) product and loses to the two fused Bluestein launches wherever those exist (padded length M <= 4096, i.e.
-    // N <= 2048: N = 34: 2.68 vs 2.03 ms, 323: 4.71 vs 1.85, 2032: 13.0 vs 1.38, 113: 10.2 vs 1.80); above that Bluestein needs
-    // 5-7 launches and the two are comparable (4416: 4.31 vs 6.54, 12167: 8.77 vs 5.90).  So a contiguous 1-D length up to 2048
+    // The Rader stage of the runtime-scheduled kernel is a direct O(p^2) product and measured slower than the two fused
+    // Bluestein launches wherever those exist (padded length M <= 4096, i.e. N <= 2048); above that Bluestein needs 5-7
+    // launches and the two are comparable.  So a contiguous 1-D length up to 2048
     // with a prime factor of 17 or more runs as Bluestein unless a curated kernel with a direct prime butterfly exists for it
     // (the {17..31} * 2^k lengths).  Factors of a Four-Step split and strided axes keep the Rader stages.
     // Round 2, later: the whole Bluestein transform in ONE launch (blue1_length: padded lengths up to 8192 in FP32, 4096 in FP64)
     // extends the rule to N <= 4096 / 2048.  B200FFT_FORCE_BLUESTEIN=1 sends every contiguous length that way
     // (tests, and A/B timing against the runtime-scheduled kernel on smooth lengths).
-    // ... and to every length whose padded transform still has the two specialised launches (FP32: padded length 8192, N <= 4096):
-    // measured against the Rader stages of the runtime-scheduled kernel (profiles/r2/bluestein_2049_4096_vs_rader.log, ms per pair
-    // of 512 MiB): N = 2050 3.15 vs 5.34, 3526 2.04 vs 9.72, 4094 1.86 vs 12.6
+    // ... and to every length whose padded transform still has the two specialised launches (FP32: padded length 8192, N <= 4096),
+    // where it also measured faster than the Rader stages of the runtime-scheduled kernel
     if (contiguous && !job.unit_lines && !dist && (N <= 2048 || blue1_length(g, N) || blue2_available(g, N)) && !(job.extra_ops & B2_OP_CONV) && !getenv("B200FFT_RADER_MAX_PRIME") &&
         !b2_find_kernel(kind, g.prec, (int)N, 0, 0)) {
         uint64_t mm = N;
@@ -784,7 +779,7 @@ int plan_c2c(PlanGraph& g, std::vector<PassPlan>& list, const C2CJob& job) {
         poor_strided = (GENERIC_SMEM_LIMIT / per_line) < 8 && N >= 64;
     }
     // specialised strided kernels with fewer than 8 neighbouring lines per CTA (N >= 4096) are slower than two
-    // launches of well-shaped ones (measured: 1950 us vs 858 + 673 us per 2 GiB pass, profiles/r1)
+    // launches of well-shaped ones (measured per 2 GiB pass)
     if (job.unit_lines) {
         const b2_kernel_info* kk = b2_find_kernel(kind, g.prec, (int)std::min<uint64_t>(N, 0x7fffffff), 0, 0);
         if (kk && kk->q < 8 && N >= 2048) poor_strided = true;

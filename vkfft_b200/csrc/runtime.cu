@@ -3,7 +3,7 @@
 // Replaces the reference's L1 "API handles" layer for the CUDA backend: table upload
 // (vkFFT_ManageLUT.h:901-915), kernel launch (vkFFT_DispatchPlan.h:157-225), buffer selection
 // (vkFFT_UpdateBuffers.h:776-1199) and teardown (vkFFT_DeletePlan.h:59-69, vkFFT_DeleteApp.h:28-324).
-// Kernels are found through the registry: compiled ahead of time for sm_100a, or -- smooth lengths outside those lists --
+// Kernels are found through the registry: compiled ahead of time for sm_90a, or -- smooth lengths outside those lists --
 // instantiated from the same templates when the plan is created (jit.cpp).  There is no CPU fallback: if the device or
 // the kernels are missing the call fails.
 #include <cuda.h>

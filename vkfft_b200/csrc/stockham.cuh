@@ -9,7 +9,7 @@
 //   so the output of the last stage is in natural order with no bit reversal.
 // What is different from the reference: twiddles are correctly-rounded LUT entries (never __sincosf),
 // thread<->line mapping can differ between the load side and the store side (so the four-step transposed
-// write is coalesced), all shapes are template constants (compiled ahead of time for sm_100a; lengths outside those lists get
+// write is coalesced), all shapes are template constants (compiled ahead of time for sm_90a; lengths outside those lists get
 // the same templates instantiated when their plan is created, jit.cpp -- there is no code GENERATOR), and the
 // inverse transform is the forward code with re/im swapped at the HBM boundary.
 #pragma once
@@ -83,7 +83,7 @@ template <typename T> B2_D cpx<T> ld_lut(const cpx<T>* p) { return *p; }
 #endif
 
 // (Streaming / evict-first hints -- __ldcs/__stcs -- on the transformed data were measured and rejected: the transposed
-//  128-byte stores lose L2 write combining and every kernel got slower, profiles/r1/README.md.)
+//  128-byte stores lose L2 write combining and every kernel got slower.)
 // two-level table lookup of W_M^m  (m = hi*2^shift + lo):  one complex multiply, error <= ~1.5 ulp
 template <typename T>
 B2_D cpx<T> twiddle2(const cpx<T>* hi, const cpx<T>* lo, uint32_t shift, uint64_t m) {
@@ -133,9 +133,7 @@ struct KCfg {
                                     : ((Sch::ns <= 1 && RMODE != 1 && RMODE != 3 && RMODE != 4) ? 0 : ((LAYOUT == LAY_LINE) ? Q * LS : N * QP));
     static constexpr int SMEM_BYTES = SMEM_ELEMS * 2 * (int)sizeof(T);
     // stage twiddles w^k generated from w^1, w^2, w^4, w^8 (Engine::compute): 4 table loads instead of 15 per radix-16
-    // butterfly.  Measured per kernel on B200: round 1 (scalar FP32) -1...-10 % for most shapes but +9 % for the contiguous
-    // 8192-point kernels; with the packed FP32 arithmetic of round 2 the 8192-point kernel gains as well (807 -> 750 us per
-    // 2 GiB pass, profiles/r2/ktune_f32_8192_twchain.log), so every kernel generates them now.
+    // butterfly; every kernel generates them.
     static constexpr bool TWCHAIN = true;
 };
 
@@ -379,9 +377,8 @@ struct Engine {
     // Two real lines (a, b) travel as one complex line a + i b.  Reading them straight into the first-stage legs
     // costs four loads per element for DCT-III (it needs p and N-p of both lines).  Instead the CTA copies both lines
     // with fully coalesced loads into the tile and the legs come from shared memory.
-    // Measured on B200 (fused DCT-III rows, N = 8192, 1 GiB of traffic): direct loads + direct scatter 599 us, staged
-    // stores only 577, staged loads only 416, both staged 394.  The DCT-II kernel keeps its direct Makhoul gather
-    // (313 us; staging its input as well: 388).
+    // Staging both the loads and the stores measured fastest for the DCT-III rows; the DCT-II kernel keeps its direct
+    // Makhoul gather, which measured faster than staging its input as well.
 #ifndef B2_TW_CHAIN
 #define B2_TW_CHAIN 1
 #endif
@@ -664,8 +661,8 @@ struct Engine {
     // outputs, three more for the step W^(line*NB) and its 2nd / 4th power, and every phase of the group is the group's
     // first one times at most three of those (error <= ~7 ulp worst case, ~2 ulp rms).  This replaced a lookup per
     // output (64 scattered 8-byte loads + 64-bit index arithmetic per 32 outputs), which kept the LSU pipe the limiter
-    // of these kernels.  Also measured on B200 and rejected (profiles/r1/README.md): a tile-factored scheme with
-    // coalesced table reads and the reference-style full M-entry table.
+    // of these kernels.  Also measured and rejected: a tile-factored scheme with coalesced table reads and the
+    // reference-style full M-entry table.
     template <int s>
     B2_D static void store_global(const X* x, XO* __restrict__ line, int64_t es_rt, int t, bool valid,
                                   const b2_pass_params& P, uint32_t gline, uint32_t qline) {
