@@ -8,6 +8,9 @@
 #include "generic.cuh"
 #include "pipe.cuh"
 #include "fused4.cuh"
+#if !defined(B2_EMU) || defined(B2_EMU_CLUSTER)
+#include "cluster4.cuh"
+#endif
 #include "ew.cuh"
 
 #if !defined(B2_EMU)
@@ -479,6 +482,109 @@ struct MaybeFused<true, T, TPLA, QA, SchA, TPLB, QB, SchB, REGS> {
 #define B2_KF(shard, T, REGS, TPLA, QA, SA, TPLB, QB, SB)                                                  \
     static ::b200fft::MaybeFused<B2_SHARD_ON(shard), T, TPLA, QA, SA, TPLB, QB, SB, REGS>                  \
         B2_CAT(b2_regf_, __COUNTER__)("FUSED4<" #T ";A " #TPLA "x" #QA " " #SA ";B " #TPLB "x" #QB " " #SB ">");
+
+// ---- cluster Four-Step (cluster4.cuh) --------------------------------------------------------------------------------
+// (the CPU emulation runs these kernels only in its build with thread-block clusters, B2_EMU_CLUSTER)
+#if !defined(B2_EMU) || defined(B2_EMU_CLUSTER)
+namespace b200fft {
+#if defined(B2_EMU)
+template <class CA, class CB, int CL, int MINB>
+int cluster_launch_impl(const b2_cluster_params* K, void*) {
+    using CK = Cluster4<CA, CB, CL>;
+    const b2_cluster_params KK = *K;
+    b2emu::launch_cluster(KK.nseq * CL, CL, CK::THREADS, CK::SMEM_BYTES, [&](unsigned char* sm) { CK::run(KK, sm); }, b2emu::st().log);
+    return emu_refused();
+}
+template <class CA, class CB, int CL, int MINB> int cluster_prepare_impl() { return 0; }
+template <class CA, class CB, int CL, int MINB> int cluster_max_active_impl(int) { return b2emu::st().cluster_capable ? 1 : 0; }
+#else
+template <class CA, class CB, int CL, int MINB>
+cudaLaunchConfig_t cluster_config(unsigned grid, cudaLaunchAttribute* at, void* stream) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(grid);
+    cfg.blockDim = dim3(Cluster4<CA, CB, CL>::THREADS);
+    cfg.dynamicSmemBytes = Cluster4<CA, CB, CL>::SMEM_BYTES;
+    cfg.stream = (cudaStream_t)stream;
+    at[0].id = cudaLaunchAttributeClusterDimension;
+    at[0].val.clusterDim.x = CL; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+    cfg.attrs = at;
+    cfg.numAttrs = 1;
+    return cfg;
+}
+template <class CA, class CB, int CL, int MINB>
+int cluster_launch_impl(const b2_cluster_params* K, void* stream) {
+    cudaLaunchAttribute at[1];
+    const cudaLaunchConfig_t cfg = cluster_config<CA, CB, CL, MINB>(K->nseq * CL, at, stream);
+    return (int)cudaLaunchKernelEx(&cfg, cluster4_kernel<CA, CB, CL, MINB>, *K);
+}
+template <class CA, class CB, int CL, int MINB>
+int cluster_prepare_impl() {
+    int rc = (int)cudaFuncSetAttribute(cluster4_kernel<CA, CB, CL, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       Cluster4<CA, CB, CL>::SMEM_BYTES);
+    if (rc == 0 && CL > 8) rc = (int)cudaFuncSetAttribute(cluster4_kernel<CA, CB, CL, MINB>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+    return rc;
+}
+// clusters the device can hold at once; 0 when it cannot run this shape at all (or there is no device)
+template <class CA, class CB, int CL, int MINB>
+int cluster_max_active_impl(int device) {
+    static int known[64] = {0};       // per device: 0 not asked yet, else 1 + the answer
+    if (device < 0 || device >= 64) return 0;
+    if (known[device]) return known[device] - 1;
+    int prev = -1;
+    if (cudaGetDevice(&prev) != cudaSuccess) { cudaGetLastError(); return 0; }
+    if (prev != device && cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); return 0; }
+    int n = 0;
+    cudaLaunchAttribute at[1];
+    const cudaLaunchConfig_t cfg = cluster_config<CA, CB, CL, MINB>(132 * CL, at, nullptr);
+    if (cluster_prepare_impl<CA, CB, CL, MINB>() != 0 ||
+        cudaOccupancyMaxActiveClusters(&n, (const void*)cluster4_kernel<CA, CB, CL, MINB>, &cfg) != cudaSuccess)
+        n = 0;
+    cudaGetLastError();
+    if (prev != device) cudaSetDevice(prev);
+    known[device] = 1 + (n > 0 ? n : 0);
+    return n > 0 ? n : 0;
+}
+#endif
+
+template <typename T, bool INV, int CL, int MINB, int TPLA, int QA, class SchA, int TPLB, int QB, class SchB>
+struct ClusterRegistrar {
+    using KA = KindTraits<B2_KIND_COLS>;
+    using KB = KindTraits<B2_KIND_ROWS_TOUT>;
+    using CA = KCfg<T, SchA, TPLA, QA, 1, KA::LMAP, KA::SMAP, KA::LAYOUT, INV, B2_OP_TWIDDLE_OUT, KA::IN_UNIT, KA::OUT_UNIT, 128, 0>;
+    using CB = KCfg<T, SchB, TPLB, QB, 1, KB::LMAP, KB::SMAP, KB::LAYOUT, INV, 0, KB::IN_UNIT, KB::OUT_UNIT, 128, 0>;
+    using CK = Cluster4<CA, CB, CL>;
+    b2_cluster_info info;
+    explicit ClusterRegistrar(const char* name) {
+        info = b2_cluster_info{};
+        info.prec = PrecOf<T>::value; info.n1 = SchA::N; info.n2 = SchB::N; info.inv = INV;
+        info.cluster = CL; info.threads = CK::THREADS; info.smem_bytes = CK::SMEM_BYTES;
+        info.tpl_a = TPLA; info.q_a = QA; info.tpl_b = TPLB; info.q_b = QB;
+        info.ns_a = SchA::ns; info.ns_b = SchB::ns;
+        for (int s = 0; s < SchA::ns; ++s) info.radices_a[s] = SchA::r(s);
+        for (int s = 0; s < SchB::ns; ++s) info.radices_b[s] = SchB::r(s);
+        info.launch = &cluster_launch_impl<CA, CB, CL, MINB>;
+        info.prepare = &cluster_prepare_impl<CA, CB, CL, MINB>;
+        info.max_active = &cluster_max_active_impl<CA, CB, CL, MINB>;
+        info.name = name;
+        b2_register_cluster(&info);
+    }
+};
+template <bool EN, typename T, int CL, int MINB, int TPLA, int QA, class SchA, int TPLB, int QB, class SchB>
+struct MaybeCluster {
+    explicit MaybeCluster(const char*) {}
+};
+template <typename T, int CL, int MINB, int TPLA, int QA, class SchA, int TPLB, int QB, class SchB>
+struct MaybeCluster<true, T, CL, MINB, TPLA, QA, SchA, TPLB, QB, SchB> {
+    ClusterRegistrar<T, false, CL, MINB, TPLA, QA, SchA, TPLB, QB, SchB> f;
+    ClusterRegistrar<T, true, CL, MINB, TPLA, QA, SchA, TPLB, QB, SchB> i;
+    explicit MaybeCluster(const char* n) : f(n), i(n) {}
+};
+}  // namespace b200fft
+//   B2_KCL(shard, type, CTAs per cluster, min CTAs per SM, TPL_A, Q_A, B2_R(radices of n1), TPL_B, Q_B, B2_R(radices of n2))
+#define B2_KCL(shard, T, CL, MINB, TPLA, QA, SA, TPLB, QB, SB)                                               \
+    static ::b200fft::MaybeCluster<B2_SHARD_ON(shard), T, CL, MINB, TPLA, QA, SA, TPLB, QB, SB>              \
+        B2_CAT(b2_regcl_, __COUNTER__)("CLUSTER4<" #T ";" #CL " CTAs;A " #TPLA "x" #QA " " #SA ";B " #TPLB "x" #QB " " #SB ">");
+#endif
 
 // short contiguous lines staged through shared memory (stockham.cuh RMODE 10): same registry key as the plain kernels
 namespace b200fft {

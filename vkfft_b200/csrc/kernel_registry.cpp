@@ -91,3 +91,42 @@ extern "C" const b2_fused_info* b2_find_fused(int prec, int n1, int n2, int inv)
 }
 extern "C" int b2_fused_count(void) { return (int)ftable().size(); }
 extern "C" const b2_fused_info* b2_fused_at(int i) { return ftable()[i]; }
+
+// ---- cluster Four-Step kernels ---------------------------------------------------------------------------------------
+namespace {
+std::vector<b2_cluster_info*>& ctable() {
+    static std::vector<b2_cluster_info*> t;
+    return t;
+}
+}  // namespace
+extern "C" void b2_register_cluster(const b2_cluster_info* k) {
+    b2_cluster_info* m = const_cast<b2_cluster_info*>(k);
+    int v = 0;
+    for (const b2_cluster_info* o : ctable())
+        if (o->prec == k->prec && o->n1 == k->n1 && o->n2 == k->n2 && o->inv == k->inv) ++v;
+    m->variant = v;
+    ctable().push_back(m);
+}
+// B200FFT_CLUSTER4_VARIANTS="n1xn2=variant,..." selects a non-default cluster shape (A/B timing)
+extern "C" const b2_cluster_info* b2_find_cluster(int prec, int n1, int n2, int inv) {
+    int v = 0;
+    if (const char* e = getenv("B200FFT_CLUSTER4_VARIANTS")) {
+        for (const char* p = e; *p;) {
+            int a, b, vv, used = 0;
+            if (sscanf(p, "%dx%d=%d%n", &a, &b, &vv, &used) == 3) {
+                if (a == n1 && b == n2) v = vv;
+                p += used;
+            } else break;
+            if (*p == ',') ++p;
+        }
+    }
+    const b2_cluster_info* dflt = nullptr;
+    for (const b2_cluster_info* k : ctable()) {
+        if (k->prec != prec || k->n1 != n1 || k->n2 != n2 || k->inv != inv) continue;
+        if (k->variant == v) return k;
+        if (k->variant == 0) dflt = k;
+    }
+    return dflt;
+}
+extern "C" int b2_cluster_count(void) { return (int)ctable().size(); }
+extern "C" const b2_cluster_info* b2_cluster_at(int i) { return ctable()[i]; }

@@ -74,6 +74,25 @@ const b2_fused_info* b2_find_fused_variant(int prec, int n1, int n2, int inv, in
 int b2_fused_count(void);
 const b2_fused_info* b2_fused_at(int i);
 
+// cluster Four-Step kernels (cluster4.cuh): both passes of n1 x n2 in one launch, one thread-block cluster per sequence
+typedef struct b2_cluster_info {
+    int prec, n1, n2, inv;             // lookup key
+    int variant;
+    int cluster, threads, smem_bytes;  // CTAs per cluster, threads per CTA, dynamic shared memory per CTA
+    int tpl_a, q_a, tpl_b, q_b;        // CTA shapes of the stand-alone kernels whose stage code the two passes run
+    int ns_a, ns_b;
+    int radices_a[8], radices_b[8];
+    int (*launch)(const b2_cluster_params* K, void* stream);
+    int (*prepare)(void);
+    // clusters of this kernel the device can hold at once (cudaOccupancyMaxActiveClusters, once per device); 0: cannot run
+    int (*max_active)(int device);
+    const char* name;
+} b2_cluster_info;
+void b2_register_cluster(const b2_cluster_info* k);
+const b2_cluster_info* b2_find_cluster(int prec, int n1, int n2, int inv);   // honours B200FFT_CLUSTER4_VARIANTS
+int b2_cluster_count(void);
+const b2_cluster_info* b2_cluster_at(int i);
+
 #ifdef __cplusplus
 }
 #endif

@@ -9,3 +9,4 @@
 #include "kernel_list_nonpow2.def"
 #include "kernel_list_blue1.def"
 #include "kernel_list_fused.def"
+#include "kernel_list_cluster.def"

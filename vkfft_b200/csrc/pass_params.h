@@ -135,6 +135,14 @@ typedef struct b2_fused_params {
     uint32_t reserved;
 } b2_fused_params;
 
+// One launch of the cluster Four-Step kernel (cluster4.cuh): both passes of N = n1*n2 with the intermediate in the distributed
+// shared memory of one thread-block cluster per sequence.  A and B are the two passes of the two-launch plan; A.out and B.in
+// (the scratch) are not touched.
+typedef struct b2_cluster_params {
+    b2_pass_params A, B;
+    uint32_t nseq;             // sequences = product of the outer extents (same for A and B); one cluster each
+} b2_cluster_params;
+
 enum {
     B2_FCTL_MAX_GROUPS = 1024,
     B2_FCTL_WORDS = 64 * B2_FCTL_MAX_GROUPS,

@@ -81,6 +81,10 @@ struct PassPlan {
     const b2_fused_info* fused = nullptr;
     uint32_t fz_nseq = 0, fz_U = 0, fz_NU = 0, fz_R = 0, fz_TA = 0, fz_TB = 0, fz_L = 1;
     int lut_id_plain = -1;       // stage tables of the stand-alone kernel `k` when lut_id belongs to the fused pair
+    // cluster Four-Step (cluster4.cuh): this launch and the NEXT one run as one launch of thread-block clusters, one per
+    // sequence (same stage tables as the two stand-alone kernels; both PassPlans stay in the list as for `fused`)
+    const b2_cluster_info* cluster = nullptr;
+    uint32_t cl_nseq = 0;
     std::string note;            // human readable (plan_describe)
 };
 

@@ -725,6 +725,53 @@ void try_fuse(PlanGraph& g, std::vector<PassPlan>& list, size_t ia) {
     b.note += " [runs inside the previous launch]";
 }
 
+// Two-factor Four-Step just emitted as list[ia] (COLS n1 + phase, -> temp) and list[ia + 1] (ROWS_TOUT n2, temp ->): run both
+// as ONE launch of thread-block clusters (cluster4.cuh), one cluster per sequence with the intermediate in distributed shared
+// memory, when a cluster kernel is registered for (n1, n2) with the very CTA shapes and radix schedules of the two kernels
+// (the results stay bit-identical to the two launches), both sides are dense FP32 complex, and the device can schedule
+// that cluster.  The opt-in L2 fusion (B200FFT_FUSED4) keeps priority.  B200FFT_NO_CLUSTER4=1 (read per plan) keeps the two
+// launches: a test hook for the bit-for-bit comparison and for A/B timing.
+void try_cluster(PlanGraph& g, std::vector<PassPlan>& list, size_t ia) {
+    const char* off = getenv("B200FFT_NO_CLUSTER4");
+    if ((off && *off && *off != '0') || ia + 2 != list.size() || half_plan(g) || g.prec != B2_PREC_F32) return;
+    PassPlan& a = list[ia];
+    PassPlan& b = list[ia + 1];
+    if (a.fused || a.sync_before || b.sync_before || a.in_scalar || b.out_scalar) return;
+    if (!a.k || !b.k || a.k->jit || b.k->jit || a.k->pipelined || b.k->pipelined || a.k->kind != B2_KIND_COLS || b.k->kind != B2_KIND_ROWS_TOUT) return;
+    if (a.k->ops != B2_OP_TWIDDLE_OUT || b.k->ops != 0 || a.k->inv != b.k->inv || a.k->v != 1 || b.k->v != 1) return;
+    const b2_cluster_info* ck = b2_find_cluster(g.prec, (int)a.P.n, (int)b.P.n, a.k->inv);
+    if (!ck) return;
+    // the stage code of exactly these two kernels
+    if (ck->tpl_a != a.k->tpl || ck->q_a != a.k->q || ck->tpl_b != b.k->tpl || ck->q_b != b.k->q || ck->ns_a != a.k->ns ||
+        ck->ns_b != b.k->ns)
+        return;
+    for (int s = 0; s < ck->ns_a; ++s) if (ck->radices_a[s] != a.k->radices[s]) return;
+    for (int s = 0; s < ck->ns_b; ++s) if (ck->radices_b[s] != b.k->radices[s]) return;
+    // one dense n1 x n2 sequence per outer coordinate: columns with unit pitch and element stride n2 in, rows transposed out
+    const int64_t n1 = a.P.n, n2 = b.P.n;
+    if (a.P.G != (uint32_t)n2 || b.P.G != (uint32_t)n1 || a.P.in_gs != 1 || a.P.in_es != n2 || b.P.out_gs != 1 || b.P.out_es != n1) return;
+    if (a.P.tw_sel != 0 || b.P.tw_sel != 0 || a.P.tw_line0 != 0) return;
+    uint64_t nseq = 1, nseq_b = 1;
+    for (int d = 0; d < B2_MAX_OUTER; ++d) { nseq *= a.P.nb[d]; nseq_b *= b.P.nb[d]; }
+    if (nseq != nseq_b || nseq * (uint64_t)ck->cluster > 0x7fffffffull) return;
+    // in place: a cluster reads its whole sequence before it writes any of it, so input and output may be the same memory
+    // only with the same layout (each sequence then overwrites exactly its own points)
+    if (a.in_role == b.out_role) {
+        if (a.in_off != b.out_off) return;
+        for (int d = 0; d < B2_MAX_OUTER; ++d)
+            if (a.P.nb[d] != b.P.nb[d] || (a.P.nb[d] > 1 && a.P.in_bs[d] != b.P.out_bs[d])) return;
+    }
+    if (ck->max_active(g.desc.device) <= 0) return;      // the device cannot hold such a cluster (or there is none)
+    a.cluster = ck;
+    a.cl_nseq = (uint32_t)nseq;
+    char buf[256];
+    snprintf(buf, sizeof buf, " [one cluster launch with the next pass: %s, clusters of %d CTAs]", ck->name, ck->cluster);
+    const size_t at = a.note.find(" n=");         // "<what> n=...": name the launch after both passes
+    if (at != std::string::npos) a.note = "four-step 1/2+2/2 in one cluster launch" + a.note.substr(at);
+    a.note += buf;
+    b.note += " [runs inside the previous launch]";
+}
+
 int plan_c2c(PlanGraph& g, std::vector<PassPlan>& list, const C2CJob& job) {
     const uint64_t N = job.N;
     const int sc_ops = (job.scale != 1.0) ? B2_OP_SCALE : 0;
@@ -921,6 +968,7 @@ int plan_c2c(PlanGraph& g, std::vector<PassPlan>& list, const C2CJob& job) {
         const size_t ia = list.size() - 1;
         if ((rc = emit(g, list, b)) != R_SUCCESS) return rc;
         if (!dist && job.tmp_base % 16 == 0) try_fuse(g, list, ia);
+        if (!dist) try_cluster(g, list, ia);
         return R_SUCCESS;
     }
     const uint64_t N1 = f[0], N2 = f[1], N3 = f[2], M = N2 * N3;

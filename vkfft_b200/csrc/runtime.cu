@@ -185,7 +185,10 @@ extern "C" int b200fft_plan_create(const b200fft_desc* desc, b200fft_plan** out)
             }
     for (int dir = 0; dir < 2 && rc == R_SUCCESS; ++dir)
         for (const PassPlan& pp : (dir ? g.inv : g.fwd))
-            if (pp.fused && pp.fused->prepare && pp.fused->prepare() != 0) { rc = R_FAILED_TO_SET_DYNAMIC_SHARED_MEMORY; break; }
+            if ((pp.fused && pp.fused->prepare && pp.fused->prepare() != 0) || (pp.cluster && pp.cluster->prepare() != 0)) {
+                rc = R_FAILED_TO_SET_DYNAMIC_SHARED_MEMORY;
+                break;
+            }
     if (rc == R_SUCCESS && g.ctl_words && cudaMalloc(&p->d_ctl, g.ctl_words * 4) != cudaSuccess) rc = R_FAILED_TO_ALLOCATE;
     // scratch for Four-Step (the reference auto-allocates tempBuffer the same way, vkFFT_InitializeApp.h:1603-1637)
     if (rc == R_SUCCESS && g.temp_elems && !g.desc.user_temp_buffer) {
@@ -293,6 +296,19 @@ static int exec_impl(b200fft_plan* p, int inverse, const b200fft_buffers* b, std
                 ++ip;
                 continue;
             }
+        }
+
+        if (pp.cluster && ip + 1 < list.size()) {
+            // both passes of a two-factor Four-Step in one launch of thread-block clusters (cluster4.cuh)
+            mark(1);
+            b2_cluster_params K;
+            memset(&K, 0, sizeof K);
+            resolve(pp, K.A);
+            resolve(list[ip + 1], K.B);
+            K.nseq = pp.cl_nseq;
+            if (pp.cluster->launch(&K, (void*)st) != 0) return fail(R_FAILED_TO_LAUNCH_KERNEL);
+            ++ip;
+            continue;
         }
 
         if (pp.sync_before) {

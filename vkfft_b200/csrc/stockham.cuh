@@ -18,7 +18,9 @@
 #include "pass_params.h"
 #include "radix.cuh"
 
-#if defined(B2_EMU)
+#if defined(B2_EMU_CLUSTER)
+#include "cuda_emu_cluster.h"       // the emulation with thread-block clusters (tests/emu/build_cluster.sh)
+#elif defined(B2_EMU)
 #include "cuda_emu.h"
 #else
 #define B2_SMEM_LD(sm, i) ((sm)[(i)])
@@ -141,7 +143,12 @@ struct KCfg {
 //   XF_LDCG      first-stage legs are read with ld.global.cg (L2 only): the data was written by other SMs during this launch
 //   XF_DISCARD   after the first-stage legs of a tile are in registers its lines are dropped from L2 without write-back
 //                (discard.global.L2): scratch that is never read again must not cost HBM write bandwidth
-enum { XF_LDCG = 1, XF_DISCARD = 2 };
+// XF (cluster Four-Step kernel, cluster4.cuh):
+//   XF_SMEM_IN   first-stage legs come from the CTA's own shared-memory tile (load_first_smem), where other CTAs of the
+//                cluster put exactly what the first launch of the two-launch plan would have written to HBM
+//   XF_DSMEM_OUT the last stage hands every output (natural-order index p, after phase / scale / inverse swap) to a sink
+//                that stores it into the shared memory of the CTA owning row p, instead of writing HBM
+enum { XF_LDCG = 1, XF_DISCARD = 2, XF_SMEM_IN = 4, XF_DSMEM_OUT = 8 };
 
 #if defined(__CUDA_ARCH__)
 // the value becomes opaque to the optimiser (it stays in its register): keeps address chains additive without losing
@@ -161,6 +168,7 @@ template <typename T> B2_D cpx<T> ld_cg(const cpx<T>* p) { return *p; }
 #endif
 
 struct NoHook { B2_D void operator()() const {} };
+struct NoSink { template <class X> B2_D void operator()(int, const X&) const {} };
 
 // ESI / ESO: compile-time element strides of the input / output lines (0 = the runtime values of the pass descriptor).
 // The fused Four-Step kernel knows both (n2 on both sides of pass A, n1 on the store side of pass B), which turns the
@@ -602,6 +610,17 @@ struct Engine {
         }
     }
 
+    // ---- XF_SMEM_IN: first-stage legs from the tile, which holds the values HBM would hold (load_global's swap included) ----
+    template <int s>
+    B2_D static void load_first_smem(X* x, const X* sm, int q, int t) {
+        static_assert((XF & XF_SMEM_IN) != 0 && s == 0 && V == 1, "first stage from shared memory");
+        load_smem<s>(x, sm, q, t);
+        if constexpr (C::INV) {
+#pragma unroll
+            for (int i = 0; i < bpt<s>() * Sch::r(s); ++i) x[i] = swp(x[i]);
+        }
+    }
+
     // ---- twiddle + butterfly ---------------------------------------------------------------------------
     template <int s>
     B2_D static void compute(X* x, const X* __restrict__ lut, int t) {
@@ -663,9 +682,10 @@ struct Engine {
     // output (64 scattered 8-byte loads + 64-bit index arithmetic per 32 outputs), which kept the LSU pipe the limiter
     // of these kernels.  Also measured and rejected: a tile-factored scheme with coalesced table reads and the
     // reference-style full M-entry table.
-    template <int s>
+    // XF_DSMEM_OUT: `line` is unused and sink(p, value) receives every output instead.
+    template <int s, class Sink = NoSink>
     B2_D static void store_global(const X* x, XO* __restrict__ line, int64_t es_rt, int t, bool valid,
-                                  const b2_pass_params& P, uint32_t gline, uint32_t qline) {
+                                  const b2_pass_params& P, uint32_t gline, uint32_t qline, const Sink& sink = Sink{}) {
         constexpr int r = Sch::r(s), NB = nbut<s>(), BPT = bpt<s>();
         static_assert(s == NS - 1, "global store only after the last stage");
         constexpr bool TW = (C::OPS & B2_OP_TWIDDLE_OUT) != 0;
@@ -713,7 +733,10 @@ struct Engine {
                     if (do_scale) a = a * sc;
                     o[v] = C::INV ? swp(a) : a;
                 }
-                if constexpr (V == 2 && C::OUT_UNIT && !HOUT) {
+                if constexpr ((XF & XF_DSMEM_OUT) != 0) {
+                    static_assert(V == 1 && !HOUT, "one output per butterfly leg, FP32 / FP64 elements");
+                    sink(b0 + k * NB, o[0]);
+                } else if constexpr (V == 2 && C::OUT_UNIT && !HOUT) {
                     using G = typename gvec<T, 2>::type;
                     G g;
                     g.x = o[0].x; g.y = o[0].y; g.z = o[1].x; g.w = o[1].y;
