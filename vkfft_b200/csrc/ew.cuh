@@ -149,11 +149,14 @@ struct Elementwise {
         } else if (P.load_io == B2_EW_CONV) {
             // (vkFFT_Convolution.h:125 does this inside the last-axis kernel)  One thread = one frequency point j of
             // input batch gl: every feature of the point is read before anything is written, so the product runs in place.
-            //   in_es / out_es = distance between feature planes of the buffer / of the kernel; in_gs = batch stride
+            //   in_es / out_es = distance between feature planes of the buffer / of the kernel, C * in_es = batch stride.
+            // A line is a whole plane (packed layout) or one row of it (padded pitches: the gaps between rows are not the
+            // transform's to touch); its place inside the batch is also its place inside every plane of the kernel.
             const uint32_t C = P.aux_u0 & 0xff, M = (P.aux_u0 >> 8) & 0xf, NK = P.aux_u1 ? P.aux_u1 : 1;
             const bool sym = (P.aux_u0 & B2_CONV_SYM) != 0, cseq = (P.aux_u0 & B2_CONV_CONJ_SEQ) != 0,
                        cker = (P.aux_u0 & B2_CONV_CONJ_KER) != 0, xps = (P.aux_u0 & B2_CONV_XPS) != 0;
-            const X* __restrict__ ker = (const X*)P.aux0;
+            const int64_t batch_stride = (int64_t)C * P.in_es;
+            const X* __restrict__ ker = (const X*)P.aux0 + in_off % batch_stride;
             const uint32_t kplanes = M >= 2 ? (sym ? M * (M + 1) / 2 : M * M) : C;
             auto finish = [&](X v) {
                 if (xps) {
@@ -181,7 +184,7 @@ struct Elementwise {
                                 if (cker) w = conj(w);
                                 acc = acc + w * x[c];
                             }
-                            out[(int64_t)k * P.out_gs + (int64_t)r * P.in_es + j] = finish(acc);
+                            out[(int64_t)k * batch_stride + (int64_t)r * P.in_es + j] = finish(acc);
                         }
                     }
                 } else {
@@ -191,7 +194,7 @@ struct Elementwise {
                         for (uint32_t k = 0; k < NK; ++k) {
                             X w = ker[(int64_t)(k * kplanes + c) * P.out_es + j];
                             if (cker) w = conj(w);
-                            out[(int64_t)k * P.out_gs + (int64_t)c * P.in_es + j] = finish(w * xv);
+                            out[(int64_t)k * batch_stride + (int64_t)c * P.in_es + j] = finish(w * xv);
                         }
                     }
                 }

@@ -1775,9 +1775,21 @@ static int build_plan_impl(const b200fft_desc& din, PlanGraph& g) {
         cv.aux_u1 = (uint32_t)NK;
         cv.in_role = cv.out_role = ROLE_BUFFER;
         cv.what = "convolution: spectrum x kernel";
-        if ((rc = emit_ew(g, g.fwd, cv, std::vector<Dim>{Dim{B, (int64_t)(C * plane), (int64_t)(C * plane)}})) != R_SUCCESS) return rc;
+        std::vector<Dim> cvl;
+        {
+            // packed layout: one line = one plane.  Padded pitches: one line = one row, so that the gaps between rows and planes
+            // (a bigger array of the caller's, for a sub-volume) are neither read nor written
+            uint64_t csize0 = d.perform_r2c ? d.size[0] / 2 + 1 : d.size[0], want = csize0;
+            bool dense = true;
+            for (uint32_t a = 0; a < d.fft_dim && dense; ++a) { dense = d.buffer_stride[a] == want; want *= (a + 1 < d.fft_dim ? d.size[a + 1] : 1); }
+            if (!dense) {
+                cv.n = (int)std::min<uint64_t>(csize0, 0x7fffffff); cv.ew_items = (uint32_t)csize0;
+                for (uint32_t a = 1; a < d.fft_dim; ++a) cvl.push_back(Dim{d.size[a], (int64_t)d.buffer_stride[a - 1], (int64_t)d.buffer_stride[a - 1]});
+            }
+        }
+        cvl.push_back(Dim{B, (int64_t)(C * plane), (int64_t)(C * plane)});      // kernel k writes output batch k (one input, NK outputs)
+        if ((rc = emit_ew(g, g.fwd, cv, cvl)) != R_SUCCESS) return rc;
         g.fwd.back().aux0_role = ROLE_KERNEL;
-        g.fwd.back().P.out_gs = (int64_t)(C * plane);     // kernel k writes output batch k (one input, NK outputs)
         // the inverse runs in `buffer` on every output batch
         b200fft_desc back = g.desc;
         g.desc.is_input_formatted = 0; g.desc.inverse_return_to_input = 0;
