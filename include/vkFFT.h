@@ -81,7 +81,7 @@ typedef struct {
 
     pfUINT doublePrecision;
     pfUINT quadDoubleDoublePrecision, quadDoubleDoublePrecisionDoubleMemory;   /* unsupported */
-    pfUINT halfPrecision;                                       /* half storage, FP32 arithmetic: plain C2C transforms */
+    pfUINT halfPrecision;                                       /* half storage, FP32 arithmetic: C2C and even-length R2C */
     pfUINT halfPrecisionMemoryOnly;                             /* half inputBuffer (isInputFormatted), FP32 everywhere else */
     pfUINT doublePrecisionFloatMemory;                          /* unsupported */
 

@@ -70,7 +70,7 @@ class VkFFTConfiguration:
     numberBatches: int = 0
     coordinateFeatures: int = 0
     doublePrecision: int = 0
-    halfPrecision: int = 0            # half-precision storage (complex32 buffers), FP32 arithmetic; plain C2C transforms
+    halfPrecision: int = 0            # half-precision storage (complex32 / float16 buffers), FP32 arithmetic; C2C, even-length R2C
     halfPrecisionMemoryOnly: int = 0  # only inputBuffer (isInputFormatted = 1) is half; buffer / tempBuffer / outputBuffer FP32
     performR2C: int = 0
     performDCT: int = 0

@@ -29,9 +29,53 @@ enum { B2_EW_COPY_MUL = 0, B2_EW_R2C_POST = 1, B2_EW_C2R_PRE = 2,
 enum { B2_CONV_SYM = 1u << 12, B2_CONV_CONJ_SEQ = 1u << 13, B2_CONV_CONJ_KER = 1u << 14, B2_CONV_XPS = 1u << 15 };
 enum { B2_EW_THREADS = 256, B2_EW_PER_THREAD = 8 };
 
-template <typename T>
+// HALF: half-precision storage on both sides (32-bit complex elements, cplx.cuh), FP32 arithmetic -- the Hermitian passes only
+// (B2_EW_R2C_POST / B2_EW_C2R_PRE of a long even-length R2C / C2R whose buffers are all half)
+template <typename T, bool HALF = false>
 struct Elementwise {
     using X = cpx<T>;
+    B2_D static X ldx(const X* p) { return *p; }
+    B2_D static X ldx(const uint32_t* p) { float re, im; b2_h2_to_f2(*p, re, im); return mk<T>((T)re, (T)im); }
+    B2_D static void stx(X* p, X a) { *p = a; }
+    B2_D static void stx(uint32_t* p, X a) { *p = b2_f2_to_h2((float)a.x, (float)a.y); }
+
+    // pairs (k, n-k), k = 0 .. n/2 ; n = P.n complex points of the half-length transform, aux0[k] = e^{-2 pi i k/(2n)}
+    template <class XS>
+    B2_D static void hermitian(const b2_pass_params& P, const XS* in, XS* out, uint32_t j0, bool do_scale, T sc) {
+        const uint32_t n = P.n;
+        const X* w = (const X*)P.aux0;
+#pragma unroll
+        for (int i = 0; i < B2_EW_PER_THREAD; ++i) {
+            const uint32_t k = j0 + i * B2_EW_THREADS;
+            if (k > n / 2) break;
+            const uint32_t kc = n - k;                    // partner index (n for k = 0)
+            if (P.load_io == B2_EW_R2C_POST) {
+                const X zk = ldx(in + (int64_t)k * P.in_es), zc = ldx(in + (int64_t)(kc == n ? 0 : kc) * P.in_es);
+                // X[k] = 1/2 (Zk + conj Zc) - i/2 w_k (Zk - conj Zc)
+                auto f = [&](X a, X bconj, X wk) {
+                    const X s = a + bconj, d = (a - bconj) * wk;
+                    X r = mk<T>(T(0.5) * (s.x + d.y), T(0.5) * (s.y - d.x));
+                    return do_scale ? r * sc : r;
+                };
+                const X xk = f(zk, conj(zc), ld_lut(w + k));
+                const X xc = f(zc, conj(zk), ld_lut(w + kc));
+                stx(out + (int64_t)k * P.out_es, xk);
+                if (kc != k) stx(out + (int64_t)kc * P.out_es, xc);
+            } else {
+                const X xk = ldx(in + (int64_t)k * P.in_es), xc = ldx(in + (int64_t)kc * P.in_es);
+                // Zin[k] = (Xk + conj Xc) + i conj(w_k) (Xk - conj Xc)
+                auto f = [&](X a, X bconj, X wk) {
+                    const X s = a + bconj, d = mulc(a - bconj, wk);
+                    return mk<T>(s.x - d.y, s.y + d.x);
+                };
+                const X zk = f(xk, conj(xc), ld_lut(w + k));
+                const X zc = f(xc, conj(xk), ld_lut(w + kc));
+                stx(out + (int64_t)k * P.out_es, zk);
+                if (kc != k && kc != n) stx(out + (int64_t)kc * P.out_es, zc);
+            }
+        }
+    }
+
     // P.load_io = operation, P.n = items per line (elements, or pairs for the R2C passes), P.tpl = chunks per line,
     // P.inverse = swap re/im right after the load, P.inner_inverse = swap right before the store.
     B2_D static void run(const b2_pass_params& P) {
@@ -44,11 +88,15 @@ struct Elementwise {
         const uint32_t o2 = rest;
         const int64_t in_off = (int64_t)o0 * P.in_bs[0] + (int64_t)o1 * P.in_bs[1] + (int64_t)o2 * P.in_bs[2] + (int64_t)gl * P.in_gs;
         const int64_t out_off = (int64_t)o0 * P.out_bs[0] + (int64_t)o1 * P.out_bs[1] + (int64_t)o2 * P.out_bs[2] + (int64_t)gl * P.out_gs;
-        const X* in = (const X*)P.in + in_off;
-        X* out = (X*)P.out + out_off;
         const T sc = (T)P.scale;
         const bool do_scale = (P.ops & B2_OP_SCALE) != 0;
         const uint32_t j0 = chunk * (B2_EW_THREADS * B2_EW_PER_THREAD) + threadIdx.x;
+        if constexpr (HALF) {
+            hermitian(P, (const uint32_t*)P.in + in_off, (uint32_t*)P.out + out_off, j0, do_scale, sc);
+            return;
+        }
+        const X* in = (const X*)P.in + in_off;
+        X* out = (X*)P.out + out_off;
         if (P.load_io == B2_EW_COPY_MUL) {
 #pragma unroll
             for (int i = 0; i < B2_EW_PER_THREAD; ++i) {
@@ -230,47 +278,15 @@ struct Elementwise {
                 }
             }
         } else {
-            // pairs (k, n-k), k = 0 .. n/2 ; n = P.n complex points of the half-length transform, aux0[k] = e^{-2 pi i k/(2n)}
-            const uint32_t n = P.n;
-            const X* w = (const X*)P.aux0;
-#pragma unroll
-            for (int i = 0; i < B2_EW_PER_THREAD; ++i) {
-                const uint32_t k = j0 + i * B2_EW_THREADS;
-                if (k > n / 2) break;
-                const uint32_t kc = n - k;                    // partner index (n for k = 0)
-                if (P.load_io == B2_EW_R2C_POST) {
-                    const X zk = in[(int64_t)k * P.in_es], zc = in[(int64_t)(kc == n ? 0 : kc) * P.in_es];
-                    // X[k] = 1/2 (Zk + conj Zc) - i/2 w_k (Zk - conj Zc)
-                    auto f = [&](X a, X bconj, X wk) {
-                        const X s = a + bconj, d = (a - bconj) * wk;
-                        X r = mk<T>(T(0.5) * (s.x + d.y), T(0.5) * (s.y - d.x));
-                        return do_scale ? r * sc : r;
-                    };
-                    const X xk = f(zk, conj(zc), ld_lut(w + k));
-                    const X xc = f(zc, conj(zk), ld_lut(w + kc));
-                    out[(int64_t)k * P.out_es] = xk;
-                    if (kc != k) out[(int64_t)kc * P.out_es] = xc;
-                } else {
-                    const X xk = in[(int64_t)k * P.in_es], xc = in[(int64_t)kc * P.in_es];
-                    // Zin[k] = (Xk + conj Xc) + i conj(w_k) (Xk - conj Xc)
-                    auto f = [&](X a, X bconj, X wk) {
-                        const X s = a + bconj, d = mulc(a - bconj, wk);
-                        return mk<T>(s.x - d.y, s.y + d.x);
-                    };
-                    const X zk = f(xk, conj(xc), ld_lut(w + k));
-                    const X zc = f(xc, conj(xk), ld_lut(w + kc));
-                    out[(int64_t)k * P.out_es] = zk;
-                    if (kc != k && kc != n) out[(int64_t)kc * P.out_es] = zc;
-                }
-            }
+            hermitian(P, in, out, j0, do_scale, sc);
         }
     }
 };
 
 #if defined(__CUDACC__)
-template <typename T>
+template <typename T, bool HALF = false>
 __global__ void __launch_bounds__(B2_EW_THREADS) elementwise_kernel(const __grid_constant__ b2_pass_params P) {
-    Elementwise<T>::run(P);
+    Elementwise<T, HALF>::run(P);
 }
 #endif
 

@@ -107,7 +107,7 @@ std::vector<int> factor(int n, bool primes) {
 
 struct Shape {
     std::vector<int> r;
-    int tpl = 0, q = 0, regs = 0, smem = 0, lut = 0, rmode_f = 0, rmode_i = 0, st = 0;
+    int tpl = 0, q = 0, regs = 0, smem = 0, smem_i = 0, lut = 0, rmode_f = 0, rmode_i = 0, st = 0;   // smem: launch size (forward kernel), smem_i: inverse kernel's own
 };
 
 // the tuned ahead-of-time kernel of the same transform (half-storage variants copy its schedule and CTA shape)
@@ -124,10 +124,12 @@ const b2_kernel_info* tuned_base(int kind, int prec, int n, int ops) {
 
 bool choose(int kind, int prec, int n, int ops_all, Shape& s) {
     const bool dbl = prec == B2_PREC_F64;
-    // half-precision storage (B2_OP_HALF_IN / _OUT -> KCfg::ST): FP32 plain complex transforms only; no ahead-of-time kernel
-    // exists for it, so every length from 2 up comes from here (one-radix kernels included)
+    // half-precision storage (B2_OP_HALF_IN / _OUT -> KCfg::ST): FP32 plain complex transforms, and the even-length R2C / C2R
+    // with half on both sides; no ahead-of-time kernel exists for it, so every length from 2 up comes from here (one-radix
+    // kernels included)
     const int half = ops_all & (B2_OP_HALF_IN | B2_OP_HALF_OUT), ops = ops_all & ~half;
-    if (half && (dbl || (ops & ~B2_OP_TWIDDLE_OUT))) return false;
+    if (half && (dbl || (ops & ~(B2_OP_TWIDDLE_OUT | B2_OP_REAL_EVEN)))) return false;
+    if (half && (ops & B2_OP_REAL_EVEN) && (kind != B2_KIND_ROWS || half != (B2_OP_HALF_IN | B2_OP_HALF_OUT))) return false;
     s.st = ((half & B2_OP_HALF_IN) ? 1 : 0) | ((half & B2_OP_HALF_OUT) ? 2 : 0);
     const b2_kernel_info* base = half ? tuned_base(kind, prec, n, ops) : nullptr;
     // contiguous FP32 lines up to 8192 points in one launch (64 KiB tile, up to 32 points per thread), everything else up to 4096
@@ -195,6 +197,7 @@ bool choose(int kind, int prec, int n, int ops_all, Shape& s) {
     const bool line = kind != B2_KIND_COLS;
     const int ls = s.q == 1 ? npad : (npad | 1);
     s.smem = s.r.size() <= 1 && !(ops & B2_OP_REAL_EVEN) ? 0 : (line ? s.q * ls : n * s.q) * esz;
+    s.smem_i = s.r.size() <= 1 ? 0 : s.smem;          // a one-radix C2R needs no tile (its Hermitian pass is in the load)
     int S = 1, lut = 0;
     for (size_t i = 0; i < s.r.size(); ++i) { if (i > 0) lut += (s.r[i] - 1) * S; S *= s.r[i]; }
     s.lut = lut;
@@ -244,7 +247,7 @@ std::string make_source(int kind, int prec, int ops, const Shape& s) {
              "    Engine<CI>::run(P, b2_smem_raw);\n"
              "}\n",
              rl.c_str(), T, s.tpl, s.q, lmap, smap, layout, ops & B2_OP_TWIDDLE_OUT, in_unit, out_unit, s.regs, s.rmode_f, s.st, T, s.tpl, s.q,
-             lmap, smap, layout, ops & B2_OP_TWIDDLE_OUT, in_unit, out_unit, s.regs, s.rmode_i, s.st, s.smem, s.smem, s.lut);
+             lmap, smap, layout, ops & B2_OP_TWIDDLE_OUT, in_unit, out_unit, s.regs, s.rmode_i, s.st, s.smem, s.smem_i, s.lut);
     return buf;
 }
 

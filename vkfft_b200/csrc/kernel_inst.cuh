@@ -119,26 +119,28 @@ struct GenericRegistrar {
 
 // ---- elementwise helper kernel ---------------------------------------------------------------------------------------
 #if defined(B2_EMU)
-template <typename T>
+template <typename T, bool HALF>
 int ew_launch(const b2_pass_params* P, unsigned grid, void*) {
     const b2_pass_params PP = *P;
-    b2emu::launch(grid, B2_EW_THREADS, 0, [&](unsigned char*) { Elementwise<T>::run(PP); }, false);
+    b2emu::launch(grid, B2_EW_THREADS, 0, [&](unsigned char*) { Elementwise<T, HALF>::run(PP); }, false);
     return emu_refused();
 }
 #else
-template <typename T>
+template <typename T, bool HALF>
 int ew_launch(const b2_pass_params* P, unsigned grid, void* stream) {
-    return launch_checked((const void*)elementwise_kernel<T>, grid, B2_EW_THREADS, 0, stream, P);
+    return launch_checked((const void*)elementwise_kernel<T, HALF>, grid, B2_EW_THREADS, 0, stream, P);
 }
 #endif
-template <typename T>
+// HALF: the half-storage Hermitian passes of long even-length R2C / C2R, registered with ops = B2_OP_HALF_IN | B2_OP_HALF_OUT
+template <typename T, bool HALF = false>
 struct ElementwiseRegistrar {
     b2_kernel_info info;
     explicit ElementwiseRegistrar(const char* name) {
         info = b2_kernel_info{};
         info.kind = B2_KIND_ELEMENTWISE; info.prec = PrecOf<T>::value;
+        info.ops = HALF ? (B2_OP_HALF_IN | B2_OP_HALF_OUT) : 0;
         info.threads = B2_EW_THREADS;
-        info.launch = &ew_launch<T>;
+        info.launch = &ew_launch<T, HALF>;
         info.name = name;
         b2_register_kernel(&info);
     }
@@ -345,6 +347,22 @@ struct MaybeHalf<true, KIND, T, TPL, Q, V, MINB, OPS, Rs...> {
 #define B2_KH(shard, KIND, OPS, TPL, Q, V, MINB, ...)                                                      \
     static ::b200fft::MaybeHalf<B2_SHARD_ON(shard), B2_KIND_##KIND, float, TPL, Q, V, MINB, OPS, __VA_ARGS__> \
         B2_CAT(b2_regh_, __COUNTER__)("HALF_" #KIND "<float," #TPL "x" #Q ",V" #V ";" #__VA_ARGS__ ">");
+// even-length R2C (forward) / C2R (inverse) on contiguous lines with half storage on both sides (the real pairs and the spectrum)
+namespace b200fft {
+template <bool EN, typename T, int TPL, int Q, int V, int MINB, int... Rs>
+struct MaybeHalfReal {
+    explicit MaybeHalfReal(const char*) {}
+};
+template <typename T, int TPL, int Q, int V, int MINB, int... Rs>
+struct MaybeHalfReal<true, T, TPL, Q, V, MINB, Rs...> {
+    Registrar<B2_KIND_ROWS, T, TPL, Q, V, MINB, false, B2_OP_REAL_EVEN | B2_OP_HALF_IN | B2_OP_HALF_OUT, Rs...> a;
+    Registrar<B2_KIND_ROWS, T, TPL, Q, V, MINB, true, B2_OP_REAL_EVEN | B2_OP_HALF_IN | B2_OP_HALF_OUT, Rs...> b;
+    explicit MaybeHalfReal(const char* n) : a(n), b(n) {}
+};
+}  // namespace b200fft
+#define B2_KHR(shard, TPL, Q, V, MINB, ...)                                                                \
+    static ::b200fft::MaybeHalfReal<B2_SHARD_ON(shard), float, TPL, Q, V, MINB, __VA_ARGS__>               \
+        B2_CAT(b2_reghr_, __COUNTER__)("HALF_R2C_ROWS<float," #TPL "x" #Q ",V" #V ";" #__VA_ARGS__ ">");
 
 // the whole Bluestein transform in one launch (stockham.cuh RMODE 11) on a palindromic schedule
 namespace b200fft {
@@ -636,3 +654,8 @@ struct MaybeStaged<true, T, Q, REGS, N> {
     static ::b200fft::MaybeSet<B2_SHARD_ON(shard), B2_KIND_##KIND, T, TPL, Q, V, MINB, \
                                __VA_ARGS__>                                                               \
         B2_CAT(b2_reg_, __COUNTER__)(#KIND "<" #T "," #TPL "x" #Q ",V" #V ";" #__VA_ARGS__ ">");
+
+// the CPU emulation (without thread-block clusters) also registers a few half-precision real kernels ahead of time
+#if defined(B2_EMU) && !defined(B2_EMU_CLUSTER)
+#include "kernel_list_emu_half.def"
+#endif

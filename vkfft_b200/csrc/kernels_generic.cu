@@ -10,3 +10,4 @@ static ::b200fft::GenericRegistrar<double, 11> b2_generic_f64_11("generic<double
 static ::b200fft::GenericRegistrar<double, 16> b2_generic_f64_16("generic<double,r<=16>");
 static ::b200fft::ElementwiseRegistrar<float> b2_ew_f32("elementwise<float>");
 static ::b200fft::ElementwiseRegistrar<double> b2_ew_f64("elementwise<double>");
+static ::b200fft::ElementwiseRegistrar<float, true> b2_ew_f32_half("elementwise<float,half in+out>");

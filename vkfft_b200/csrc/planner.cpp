@@ -464,8 +464,12 @@ int plan_c2c(PlanGraph& g, std::vector<PassPlan>& list, const C2CJob& job);
 
 // elementwise helper launch over `lines` (every line dimension, any order)
 int emit_ew(PlanGraph& g, std::vector<PassPlan>& list, PassReq rq, const std::vector<Dim>& lines) {
-    const b2_kernel_info* k = b2_find_kernel(B2_KIND_ELEMENTWISE, g.prec, 0, 0, 0);
-    if (!k || g.role_half[rq.in_role] || g.role_half[rq.out_role]) return R_UNSUPPORTED_FFT_LENGTH;
+    // half-precision storage: only the Hermitian passes of a long even-length R2C / C2R, half on both sides
+    const bool half_in = g.role_half[rq.in_role], half_out = g.role_half[rq.out_role];
+    const bool half = half_in && half_out && (rq.ew_op == 1 || rq.ew_op == 2);   // B2_EW_R2C_POST, B2_EW_C2R_PRE
+    if ((half_in || half_out) && !half) return R_UNSUPPORTED_FFT_LENGTH;
+    const b2_kernel_info* k = b2_find_kernel(B2_KIND_ELEMENTWISE, g.prec, 0, 0, half ? (B2_OP_HALF_IN | B2_OP_HALF_OUT) : 0);
+    if (!k) return R_UNSUPPORTED_FFT_LENGTH;
     std::vector<Dim> m = merge_dims(lines);
     if (m.size() > 1 + B2_MAX_OUTER) return R_UNSUPPORTED_FFT_LENGTH;
     PassPlan pp;
@@ -495,7 +499,7 @@ int emit_ew(PlanGraph& g, std::vector<PassPlan>& list, PassReq rq, const std::ve
     pp.lut_id = lut_for(g, std::vector<int>{});
     pp.aux0_id = rq.aux0; pp.aux1_id = rq.aux1;
     char buf[200];
-    snprintf(buf, sizeof buf, "%s elementwise op=%d items=%u grid=%u", rq.what, rq.ew_op, rq.ew_items, pp.grid);
+    snprintf(buf, sizeof buf, "%s elementwise op=%d items=%u grid=%u%s", rq.what, rq.ew_op, rq.ew_items, pp.grid, half ? " half in+out" : "");
     pp.note = buf;
     list.push_back(pp);
     return R_SUCCESS;
@@ -1167,8 +1171,15 @@ int plan_direction_r2c(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
             if (!d.omit_dimension[a]) norm /= (double)d.size[a];
     const bool even = (N0 % 2 == 0) && N0 > 2;   // N0 = 2 has no half-length transform: it takes the zero-imaginary path of the odd lengths
     const uint64_t n = even ? N0 / 2 : N0;
-    const bool fused = n >= 2 && ((is_smooth(n) && generic_fits(g, n)) ||
-                                  (even && b2_find_kernel(B2_KIND_ROWS, g.prec, (int)n, 0, B2_OP_REAL_EVEN) != nullptr));
+    // half-precision storage: only the even lengths, whose real samples are addressed in pairs (one 32-bit element), and only
+    // where the half-length C2C has a half plan.  The runtime-scheduled kernel has no half variant, so a length without a fused
+    // half kernel runs as the half-length C2C + the half Hermitian launch, and fails where that C2C does (Bluestein lengths,
+    // among them the bare primes 17...31, which a C2C plan sends to Bluestein although a one-radix kernel exists)
+    const bool half = half_plan(g);
+    if (half && (!even || n == 17 || n == 19 || n == 23 || n == 29 || n == 31)) return R_UNSUPPORTED_FFT_LENGTH_R2C;
+    const int hops = half ? (B2_OP_HALF_IN | B2_OP_HALF_OUT) : 0;
+    const bool fused = n >= 2 && ((!half && is_smooth(n) && generic_fits(g, n)) ||
+                                  (even && b2_find_kernel(B2_KIND_ROWS, g.prec, (int)n, 0, B2_OP_REAL_EVEN | hops) != nullptr));
     const bool odd_composed = !fused && !even && n >= 3;   // long / non-smooth odd lengths: C2C plan on scratch + copy launches
     if (!fused && !even && !odd_composed) return R_UNSUPPORTED_FFT_LENGTH_R2C;
 
@@ -1200,7 +1211,7 @@ int plan_direction_r2c(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
         rq.outer = m;
         rq.in_es = 1; rq.out_es = 1;
         // specialised kernel with the Hermitian pass fused in (one HBM round trip, registers + shared memory)
-        if (even && b2_find_kernel(B2_KIND_ROWS, g.prec, (int)n, forward ? 0 : 1, B2_OP_REAL_EVEN)) {
+        if (even && b2_find_kernel(B2_KIND_ROWS, g.prec, (int)n, forward ? 0 : 1, B2_OP_REAL_EVEN | hops)) {
             rq.force_generic = false;
             rq.inv = forward ? 0 : 1;
             rq.ops = B2_OP_REAL_EVEN | ((!forward && scale != 1.0) ? B2_OP_SCALE : 0);
@@ -1248,14 +1259,15 @@ int plan_direction_r2c(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
         int r;
         if (forward) {
             job.inv = 0; job.in_role = real_role; job.out_role = ROLE_BUFFER; job.scale = 1.0;
-            if ((r = plan_c2c(g, list, job)) != R_SUCCESS) return r;
+            if ((r = plan_c2c(g, list, job)) != R_SUCCESS) return half ? R_UNSUPPORTED_FFT_LENGTH_R2C : r;
             ew.ew_op = 1; ew.what = "r2c hermitian pass";
             return emit_ew(g, list, ew, cc_lines);
         }
         ew.ew_op = 2; ew.what = "c2r hermitian pass";
         if ((r = emit_ew(g, list, ew, cc_lines)) != R_SUCCESS) return r;
         job.inv = 1; job.in_role = ROLE_BUFFER; job.out_role = real_role; job.scale = scale;
-        return plan_c2c(g, list, job);
+        r = plan_c2c(g, list, job);
+        return (r != R_SUCCESS && half) ? R_UNSUPPORTED_FFT_LENGTH_R2C : r;
     };
     // odd lengths the single-launch kernel cannot take (prime factors above 127, or too long for shared memory): the real
     // lines are widened to complex lines in scratch, transformed by an ordinary C2C plan (Bluestein / Four-Step as needed)
@@ -1584,10 +1596,11 @@ static int build_plan_impl(const b200fft_desc& din, PlanGraph& g) {
     // transform first reads and where the inverse transform last writes): the caller's inputBuffer is half, buffer / tempBuffer /
     // outputBuffer are FP32 -- forward inputBuffer -> buffer, inverse (inverseReturnToInputBuffer) buffer -> inputBuffer
     if (d.precision == B200FFT_F16_IO && !d.is_input_formatted) return R_UNSUPPORTED_FFT_LENGTH;
-    // half-precision storage: plain complex transforms (the conversion is fused into the first-stage load / last-stage store of the
-    // specialised kernels); the real-data operators, convolution and zero padding have no half variant
-    if ((d.precision == B200FFT_F16 || d.precision == B200FFT_F16_IO) && (d.perform_r2c || d.perform_dct || d.perform_dst || d.perform_convolution || d.dist_world > 1))
+    // half-precision storage: complex transforms and (halfPrecision only) even-length R2C / C2R -- the conversion is fused into the
+    // first-stage load / last-stage store of the specialised kernels; DCT / DST, convolution and zero padding have no half variant
+    if ((d.precision == B200FFT_F16 || d.precision == B200FFT_F16_IO) && (d.perform_dct || d.perform_dst || d.perform_convolution || d.dist_world > 1))
         return R_UNSUPPORTED_FFT_LENGTH;
+    if (d.precision == B200FFT_F16_IO && d.perform_r2c) return R_UNSUPPORTED_FFT_LENGTH;
     if (d.perform_dct > 4 || d.perform_dst > 4) return R_UNSUPPORTED_FFT_LENGTH_R2R;
     if ((d.perform_r2c && (d.perform_dct || d.perform_dst)) || (d.perform_dct && d.perform_dst)) return R_UNSUPPORTED_FFT_LENGTH_R2R;
     if (d.omit_dimension[0] && d.perform_r2c) return R_UNSUPPORTED_FFT_OMIT;

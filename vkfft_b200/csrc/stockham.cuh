@@ -100,7 +100,8 @@ template <typename T_, class Sch_, int TPL_, int Q_, int V_, int LMAP_, int SMAP
           int OPS_, bool IN_UNIT_, bool OUT_UNIT_, int REGS_ = 128, int RMODE_ = 0, int ST_ = 0>
 struct KCfg {
     // storage in HBM: 0 = elements of T on both sides; bit 0 = the lines READ are half precision (32-bit complex elements),
-    // bit 1 = the lines WRITTEN are (cplx.cuh; plain complex transforms only).  Strides and offsets count elements either way
+    // bit 1 = the lines WRITTEN are (cplx.cuh; plain complex transforms, and even-length R2C / C2R with both bits set, where a
+    // pair of half reals is one 32-bit element).  Strides and offsets count elements either way
     static constexpr int ST = ST_;
     using T = T_;
     using Sch = Sch_;
@@ -183,7 +184,9 @@ struct Engine {
     static constexpr bool RUNNING_OUT = !C::OUT_UNIT && ESO == 0;
     // element types in HBM (half-precision storage: one 32-bit word per complex element, converted in the load / store)
     static constexpr bool HIN = (C::ST & 1) != 0, HOUT = (C::ST & 2) != 0;
-    static_assert(C::ST == 0 || (C::RMODE == 0 && V == 1 && sizeof(T) == 4 && XF == 0), "half storage: plain FP32 complex transforms");
+    // (even-length R2C / C2R: half on both sides only -- the real pairs and the spectrum are both 32-bit elements)
+    static_assert(C::ST == 0 || ((C::RMODE == 0 || ((C::RMODE == 1 || C::RMODE == 2) && C::ST == 3)) && V == 1 && sizeof(T) == 4 && XF == 0),
+                  "half storage: FP32 complex transforms and even-length real transforms");
     template <bool H, class A, class B> struct Sel { using type = A; };
     template <class A, class B> struct Sel<true, A, B> { using type = B; };
     using XI = typename Sel<HIN, X, uint32_t>::type;
@@ -250,7 +253,7 @@ struct Engine {
     // ---- C2R: first-stage legs assembled from the Hermitian half spectrum (n+1 inputs per line) ---------------------
     //  Zin[p] = (X[p] + conj X[n-p]) + i conj(w_p) (X[p] - conj X[n-p]),  w_p = e^{-2 pi i p/2n};  then the inverse FFT
     template <int s>
-    B2_D static void load_global_c2r(X* x, const X* __restrict__ line, const X* __restrict__ w, int t, bool valid) {
+    B2_D static void load_global_c2r(X* x, const XI* __restrict__ line, const X* __restrict__ w, int t, bool valid) {
         constexpr int r = Sch::r(s), NB = nbut<s>(), BPT = bpt<s>();
 #pragma unroll
         for (int m = 0; m < BPT; ++m) {
@@ -263,7 +266,7 @@ struct Engine {
                     const int p = b + k * NB;
                     X z = mk<T>(T(0), T(0));
                     if (ok) {
-                        const X a = line[p], bc = conj(line[N - p]);
+                        const X a = ldx(line + p), bc = conj(ldx(line + (N - p)));
                         const X sm = a + bc, d = mulc(a - bc, ld_lut(w + p));
                         z = mk<T>(sm.x - d.y, sm.y + d.x);
                     }
@@ -567,7 +570,7 @@ struct Engine {
     // ---- R2C: Hermitian post-pass through shared memory, n+1 outputs per line ---------------------------------------
     //  X[k] = 1/2 (Z[k] + conj Z[n-k]) - i/2 w_k (Z[k] - conj Z[n-k])
     template <int s>
-    B2_D static void store_global_r2c(const X* x, X* sm, X* __restrict__ line, const X* __restrict__ w, int q, int t,
+    B2_D static void store_global_r2c(const X* x, X* sm, XO* __restrict__ line, const X* __restrict__ w, int q, int t,
                                       bool valid, const b2_pass_params& P) {
         constexpr int r = Sch::r(s), NB = nbut<s>(), BPT = bpt<s>();
         const bool do_scale = (P.ops & B2_OP_SCALE) != 0;
@@ -590,7 +593,7 @@ struct Engine {
             const X sum = a + bc, d = (a - bc) * ld_lut(w + k);
             X o = mk<T>(T(0.5) * (sum.x + d.y), T(0.5) * (sum.y - d.x));
             if (do_scale) o = o * sc;
-            line[k] = o;
+            stx(line + k, o);
         }
     }
 

@@ -15,6 +15,12 @@ This module gives the same surface over the C ABI:
 `norm`: 0 = nothing (the library's own convention: unnormalised inverse), 1 = backward transform scaled by 1/N (numpy's
 default), "ortho" = both directions scaled by 1/sqrt(N).  Plans are cached per configuration; tensors must be contiguous.
 PyTorch is used for device memory only.
+
+Precision follows the dtype: complex64 / float32 (FP32), complex128 / float64 (FP64), and complex32 / float16 for
+fftn / ifftn / rfftn / irfftn (halfPrecision: half storage, FP32 arithmetic).  The cosine / sine transforms take float32
+and float64 only; any other dtype (bfloat16, integers, half DCT / DST) raises TypeError before anything is planned.
+A half inverse with norm=1 is scaled in FP32 inside the transform (the plan's `normalize`): scaled afterwards, the
+unnormalised result would leave half's range at modest sizes.
 """
 import math
 from typing import Dict, Optional, Tuple
@@ -61,11 +67,31 @@ def _stream(torch, cuda_stream):
     return cuda_stream if cuda_stream is not None else torch.cuda.current_stream().cuda_stream
 
 
-def _scale_after(t, n, norm, inverse):
+# VkFFTConfiguration precision of each dtype: 0 FP32, 1 FP64, 2 half storage
+_COMPLEX_PREC = {"complex64": 0, "complex128": 1, "complex32": 2}
+_REAL_PREC = {"float32": 0, "float64": 1, "float16": 2}
+
+
+def _prec(t, table, what):
+    p = table.get(str(t.dtype).replace("torch.", ""))
+    if p is None:
+        raise TypeError(f"{what}: unsupported dtype {t.dtype} (supported: {', '.join(table)})")
+    return p
+
+
+def _prec_cfg(prec, norm):
+    """configuration keys of a precision; half plans apply norm=1 themselves (normalize = 1 on the inverse)"""
+    return {"doublePrecision": int(prec == 1), "halfPrecision": int(prec == 2), "normalize": int(prec == 2 and norm == 1)}
+
+
+def _scale_after(t, n, norm, inverse, prec=0):
+    import torch
     if norm == "ortho":
-        t.mul_(1.0 / math.sqrt(n))
+        # complex32 has no multiply: scale its float16 view
+        (torch.view_as_real(t) if prec == 2 and t.is_complex() else t).mul_(1.0 / math.sqrt(n))
     elif norm == 1 and inverse:
-        t.mul_(1.0 / n)
+        if prec != 2:                          # half: already scaled by the plan
+            t.mul_(1.0 / n)
     elif norm not in (0, 1, "ortho"):
         raise ValueError("norm must be 0, 1 or 'ortho'")
 
@@ -81,6 +107,7 @@ def _c2c(src, dest, ndim, norm, cuda_stream, inverse):
     _check(src, "src")
     if not src.is_complex():
         raise TypeError("complex tensor expected; use rfftn for real input")
+    prec = _prec(src, _COMPLEX_PREC, "fftn / ifftn")
     inplace = dest is not None and dest.data_ptr() == src.data_ptr()
     if dest is None:
         dest = torch.empty_like(src)
@@ -88,7 +115,6 @@ def _c2c(src, dest, ndim, norm, cuda_stream, inverse):
     if dest.shape != src.shape or dest.dtype != src.dtype:
         raise ValueError("dest must match src")
     nd, sizes, batch = _split(src.shape, ndim)
-    dbl = src.dtype == torch.complex128
     dev = src.device.index
     if all(s == 1 for s in sizes):
         # every transformed axis has one point: the plan has no launch (plan_direction_c2c skips such axes), so an
@@ -101,8 +127,9 @@ def _c2c(src, dest, ndim, norm, cuda_stream, inverse):
     # leave the result in `buffer`
     fmt = {} if inplace else ({"isOutputFormatted": 1, "makeInversePlanOnly": 1} if inverse else
                               {"isInputFormatted": 1, "makeForwardPlanOnly": 1})
-    app = _plan(("c2c", tuple(sizes), batch, dbl, dev, inplace, inverse and not inplace), FFTdim=nd, size=sizes,
-                numberBatches=batch, device=dev, doublePrecision=int(dbl), **fmt)
+    pc = _prec_cfg(prec, norm)
+    app = _plan(("c2c", tuple(sizes), batch, prec, pc["normalize"], dev, inplace, inverse and not inplace), FFTdim=nd, size=sizes,
+                numberBatches=batch, device=dev, **pc, **fmt)
     lp = api.VkFFTLaunchParams(buffer=dest, stream=_stream(torch, cuda_stream))
     if not inplace:
         if inverse:
@@ -115,7 +142,7 @@ def _c2c(src, dest, ndim, norm, cuda_stream, inverse):
     n = 1
     for s in sizes:
         n *= s
-    _scale_after(dest, n, norm, inverse)
+    _scale_after(dest, n, norm, inverse, prec)
     return dest
 
 
@@ -135,9 +162,9 @@ def rfftn(src, dest=None, ndim=None, norm=1, cuda_stream=None):
     _check(src, "src")
     if src.is_complex():
         raise TypeError("real tensor expected")
+    prec = _prec(src, _REAL_PREC, "rfftn")
     nd, sizes, batch = _split(src.shape, ndim)
-    dbl = src.dtype == torch.float64
-    cdt = torch.complex128 if dbl else torch.complex64
+    cdt = (torch.complex64, torch.complex128, torch.complex32)[prec]
     oshape = tuple(src.shape[:-1]) + (src.shape[-1] // 2 + 1,)
     if dest is None:
         dest = torch.empty(oshape, dtype=cdt, device=src.device)
@@ -145,15 +172,16 @@ def rfftn(src, dest=None, ndim=None, norm=1, cuda_stream=None):
     if tuple(dest.shape) != oshape or dest.dtype != cdt:
         raise ValueError(f"dest must be {oshape} {cdt}")
     dev = src.device.index
-    app = _plan(("r2c", tuple(sizes), batch, dbl, dev), FFTdim=nd, size=sizes, numberBatches=batch, device=dev,
-                doublePrecision=int(dbl), performR2C=1, isInputFormatted=1, inverseReturnToInputBuffer=1)
+    pc = _prec_cfg(prec, norm)
+    app = _plan(("r2c", tuple(sizes), batch, prec, pc["normalize"], dev), FFTdim=nd, size=sizes, numberBatches=batch, device=dev,
+                performR2C=1, isInputFormatted=1, inverseReturnToInputBuffer=1, **pc)
     rc = api.VkFFTAppend(app, -1, api.VkFFTLaunchParams(buffer=dest, inputBuffer=src, stream=_stream(torch, cuda_stream)))
     if rc != 0:
         raise RuntimeError("VkFFTAppend: " + api.getVkFFTErrorString(rc))
     n = 1
     for s in sizes:
         n *= s
-    _scale_after(dest, n, norm, False)
+    _scale_after(dest, n, norm, False, prec)
     return dest
 
 
@@ -165,12 +193,12 @@ def irfftn(src, dest=None, ndim=None, norm=1, cuda_stream=None, n_last=None):
     _check(src, "src")
     if not src.is_complex():
         raise TypeError("complex tensor expected")
+    prec = _prec(src, _COMPLEX_PREC, "irfftn")
     n_last = 2 * (src.shape[-1] - 1) if n_last is None else n_last
     if n_last // 2 + 1 != src.shape[-1]:
         raise ValueError("n_last does not match the Hermitian axis")
     rshape = tuple(src.shape[:-1]) + (n_last,)
-    dbl = src.dtype == torch.complex128
-    rdt = torch.float64 if dbl else torch.float32
+    rdt = (torch.float32, torch.float64, torch.float16)[prec]
     if dest is None:
         dest = torch.empty(rshape, dtype=rdt, device=src.device)
     _check(dest, "dest")
@@ -178,15 +206,16 @@ def irfftn(src, dest=None, ndim=None, norm=1, cuda_stream=None, n_last=None):
         raise ValueError(f"dest must be {rshape} {rdt}")
     nd, sizes, batch = _split(rshape, ndim)
     dev = src.device.index
-    app = _plan(("r2c", tuple(sizes), batch, dbl, dev), FFTdim=nd, size=sizes, numberBatches=batch, device=dev,
-                doublePrecision=int(dbl), performR2C=1, isInputFormatted=1, inverseReturnToInputBuffer=1)
+    pc = _prec_cfg(prec, norm)
+    app = _plan(("r2c", tuple(sizes), batch, prec, pc["normalize"], dev), FFTdim=nd, size=sizes, numberBatches=batch, device=dev,
+                performR2C=1, isInputFormatted=1, inverseReturnToInputBuffer=1, **pc)
     rc = api.VkFFTAppend(app, 1, api.VkFFTLaunchParams(buffer=src, inputBuffer=dest, stream=_stream(torch, cuda_stream)))
     if rc != 0:
         raise RuntimeError("VkFFTAppend: " + api.getVkFFTErrorString(rc))
     n = 1
     for s in sizes:
         n *= s
-    _scale_after(dest, n, norm, True)
+    _scale_after(dest, n, norm, True, prec)
     return dest
 
 
@@ -196,17 +225,17 @@ def _r2r(src, dest, ndim, norm, cuda_stream, inverse, kind, dst):
     _check(src, "src")
     if src.is_complex():
         raise TypeError("real tensor expected")
+    prec = _prec(src, {k: v for k, v in _REAL_PREC.items() if v != 2}, "dctn / dstn")    # no half cosine / sine transforms
     if dest is None:
         dest = src.clone()
     elif dest.data_ptr() != src.data_ptr():
         _check(dest, "dest")
         dest.copy_(src)
     nd, sizes, batch = _split(src.shape, ndim)
-    dbl = src.dtype == torch.float64
     dev = src.device.index
     name = "performDST" if dst else "performDCT"
-    app = _plan((name, kind, tuple(sizes), batch, dbl, dev), FFTdim=nd, size=sizes, numberBatches=batch, device=dev,
-                doublePrecision=int(dbl), **{name: kind})
+    app = _plan((name, kind, tuple(sizes), batch, prec, dev), FFTdim=nd, size=sizes, numberBatches=batch, device=dev,
+                doublePrecision=int(prec == 1), **{name: kind})
     rc = api.VkFFTAppend(app, 1 if inverse else -1, api.VkFFTLaunchParams(buffer=dest, stream=_stream(torch, cuda_stream)))
     if rc != 0:
         raise RuntimeError("VkFFTAppend: " + api.getVkFFTErrorString(rc))
