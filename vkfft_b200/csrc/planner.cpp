@@ -443,6 +443,9 @@ struct C2CJob {
     // distributed N-D transform, the axis that crosses the slabs: this rank transforms 1/line_world of the lines (a slice
     // of the outermost line dimension); its strided loads and stores reach into every rank's slab of the peer window
     uint32_t line_world = 1, line_rank = 0;
+    // R2C slab plans: when no line dimension divides by line_world, the first one (the H = nx/2+1 spectrum columns) is cut
+    // into contiguous ranges on multiples of 8 columns and the last rank takes the remainder
+    bool line_ragged = false;
     bool sync_first = false;            // a barrier over all ranks precedes the first launch of this job
     // fused convolution along this axis (single launch only): B2_OP_CONV + its operands
     int extra_ops = 0;
@@ -788,6 +791,17 @@ int plan_c2c(PlanGraph& g, std::vector<PassPlan>& list, const C2CJob& job) {
             uint64_t first;
             if (sliced[i].n > 1 && sliced[i].n % job.line_world == 0) done = slice_dim(sliced[i], job.line_world, job.line_rank, slice_in, slice_out, first);
         }
+        if (!done && job.line_ragged && !sliced.empty()) {
+            Dim& c = sliced[0];
+            uint64_t per = c.n / job.line_world;
+            if (per >= 8) per &= ~7ull;          // range boundaries on whole 8-column groups (neighbouring lanes of one CTA)
+            if (per == 0) return R_UNSUPPORTED_FFT_LENGTH;
+            const uint64_t first = (uint64_t)job.line_rank * per;
+            c.n = (job.line_rank + 1 == job.line_world) ? c.n - first : per;
+            slice_in += (int64_t)first * c.is;
+            slice_out += (int64_t)first * c.os;
+            done = true;
+        }
         if (!done) return R_UNSUPPORTED_FFT_LENGTH;
     }
     std::vector<Dim> m = merge_dims(sliced);
@@ -1054,6 +1068,15 @@ std::vector<Dim> other_dims(const PlanGraph& g, const uint64_t* size, uint32_t a
     return lines;
 }
 
+// distributed N-D plan: first element of this rank's slab in `buffer` and in scratch (both windows have the same slabs).
+// Rank g owns indices [g*n/R, (g+1)*n/R) of the last dimension, so its slab starts g*n/R outermost pitches in -- for R2C
+// the pitches of the complex rows, which may be padded so that a slab fills whole mapping granules
+int64_t slab_base(const PlanGraph& g) {
+    const b200fft_desc& d = g.desc;
+    const uint32_t la = d.fft_dim - 1;
+    return (int64_t)((uint64_t)d.dist_rank * (d.size[la] / d.dist_world) * d.buffer_stride[la - 1]);
+}
+
 // slab: < 0 ordinary plan;  0: local axis of a distributed N-D plan (this rank's slab only: `size` already holds the slab's
 // extent of the last dimension, every base moves to the slab);  1: the axis that crosses the slabs (lines shared out over the ranks)
 int plan_c2c_axis(PlanGraph& g, std::vector<PassPlan>& list, const uint64_t* size, uint32_t axis, int inv,
@@ -1070,10 +1093,10 @@ int plan_c2c_axis(PlanGraph& g, std::vector<PassPlan>& list, const uint64_t* siz
     if (slab < 0) {
         if (g.distributed) { job.world = g.desc.dist_world; job.rank = g.desc.dist_rank; }
     } else if (slab == 0) {
-        const int64_t base = (int64_t)((uint64_t)g.desc.dist_rank * (g.total_elems / g.desc.dist_world));
-        job.in_base = job.out_base = job.tmp_base = base;
+        job.in_base = job.out_base = job.tmp_base = slab_base(g);
     } else {
         job.line_world = g.desc.dist_world; job.line_rank = g.desc.dist_rank;
+        job.line_ragged = g.desc.perform_r2c != 0;
     }
     return plan_c2c(g, list, job);
 }
@@ -1164,7 +1187,15 @@ int plan_direction_r2c(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
     uint64_t csize[B200FFT_MAX_DIMS];
     for (int a = 0; a < B200FFT_MAX_DIMS; ++a) csize[a] = d.size[a];
     csize[0] = H;                       // the other axes transform H columns (vkFFT_Scheduler.h:2281-2283)
-    const Layout buf = layout_of(ROLE_BUFFER, d.buffer_stride, d.fft_dim);
+    // distributed (slabs along the last dimension): the x axis and, in 3-D, the y axis run on this rank's slab only
+    uint64_t rsize[B200FFT_MAX_DIMS], lcsize[B200FFT_MAX_DIMS];
+    for (int a = 0; a < B200FFT_MAX_DIMS; ++a) { rsize[a] = d.size[a]; lcsize[a] = csize[a]; }
+    const uint32_t la = d.fft_dim - 1;
+    const int64_t base = g.distributed ? slab_base(g) : 0;
+    if (g.distributed) { rsize[la] /= d.dist_world; lcsize[la] /= d.dist_world; }
+    Layout buf = layout_of(ROLE_BUFFER, d.buffer_stride, d.fft_dim);
+    // one batch: its pitch addresses nothing, but sizes the scratch of a Four-Step -- a slab's worth, not the whole window
+    if (g.distributed) buf.batch_stride = rsize[la] * d.buffer_stride[la - 1];
     double norm = 1.0;
     if (inv && d.normalize)
         for (uint32_t a = 0; a < d.fft_dim; ++a)
@@ -1189,7 +1220,7 @@ int plan_direction_r2c(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
     // strides of the real rows in REAL elements
     uint64_t rstride[B200FFT_MAX_DIMS];
     for (int a = 0; a < B200FFT_MAX_DIMS; ++a) rstride[a] = real_ext ? d.input_stride[a] : 2 * d.buffer_stride[a];
-    const uint64_t rbatch = rstride[d.fft_dim - 1];
+    const uint64_t rbatch = g.distributed ? 2 * buf.batch_stride : rstride[d.fft_dim - 1];
     if (even)
         for (uint32_t a = 0; a < d.fft_dim; ++a)
             if (rstride[a] % 2) return R_UNSUPPORTED_FFT_LENGTH_R2C;
@@ -1201,7 +1232,7 @@ int plan_direction_r2c(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
         std::vector<Dim> lines;
         for (uint32_t a = 1; a < d.fft_dim; ++a) {
             const int64_t rs = (int64_t)(rstride[a - 1] / unit), cs = (int64_t)d.buffer_stride[a - 1];
-            lines.push_back(forward ? Dim{d.size[a], rs, cs} : Dim{d.size[a], cs, rs});
+            lines.push_back(forward ? Dim{rsize[a], rs, cs} : Dim{rsize[a], cs, rs});
         }
         lines.push_back(forward ? Dim{g.batches, (int64_t)(rbatch / unit), (int64_t)buf.batch_stride}
                                 : Dim{g.batches, (int64_t)buf.batch_stride, (int64_t)(rbatch / unit)});
@@ -1210,6 +1241,7 @@ int plan_direction_r2c(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
         else { rq.group = m[0]; m.erase(m.begin()); }
         rq.outer = m;
         rq.in_es = 1; rq.out_es = 1;
+        rq.in_base = rq.out_base = base;   // in place: the real pairs and the spectrum start at the same element
         // specialised kernel with the Hermitian pass fused in (one HBM round trip, registers + shared memory)
         if (even && b2_find_kernel(B2_KIND_ROWS, g.prec, (int)n, forward ? 0 : 1, B2_OP_REAL_EVEN | hops)) {
             rq.force_generic = false;
@@ -1244,8 +1276,8 @@ int plan_direction_r2c(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
         std::vector<Dim> rc_lines, cc_lines;   // real(complex view)->complex and complex->complex line dims
         for (uint32_t a = 1; a < d.fft_dim; ++a) {
             const int64_t rs = (int64_t)(rstride[a - 1] / 2), cs = (int64_t)d.buffer_stride[a - 1];
-            rc_lines.push_back(forward ? Dim{d.size[a], rs, cs} : Dim{d.size[a], cs, rs});
-            cc_lines.push_back(Dim{d.size[a], cs, cs});
+            rc_lines.push_back(forward ? Dim{rsize[a], rs, cs} : Dim{rsize[a], cs, rs});
+            cc_lines.push_back(Dim{rsize[a], cs, cs});
         }
         rc_lines.push_back(forward ? Dim{g.batches, (int64_t)(rbatch / 2), (int64_t)buf.batch_stride}
                                    : Dim{g.batches, (int64_t)buf.batch_stride, (int64_t)(rbatch / 2)});
@@ -1254,8 +1286,10 @@ int plan_direction_r2c(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
         ew.elementwise = true; ew.ew_items = (uint32_t)(n / 2 + 1); ew.n = (int)n;
         ew.in_es = ew.out_es = 1; ew.in_role = ew.out_role = ROLE_BUFFER;
         ew.aux0 = aux_for(g, AUX_R2C, N0);
+        ew.in_base = ew.out_base = base;
         C2CJob job;
         job.N = n; job.es_in = job.es_out = 1; job.lines = rc_lines; job.unit_lines = false;
+        job.in_base = job.out_base = job.tmp_base = base;
         int r;
         if (forward) {
             job.inv = 0; job.in_role = real_role; job.out_role = ROLE_BUFFER; job.scale = 1.0;
@@ -1322,6 +1356,40 @@ int plan_direction_r2c(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
     int rc;
     size_t mark = list.size();
     auto count = [&](uint32_t a) { g.axis_uploads[inv ? 1 : 0][a] += (uint32_t)(list.size() - mark); mark = list.size(); };
+    if (g.distributed) {
+        // Slabs along the last dimension (DESIGN section 7): x (and y) inside this rank's slab, then -- after a barrier -- the
+        // last axis as strided launches over the whole window on this rank's share of the H*ny spectrum columns; the inverse
+        // runs the other way round.  Whatever scratch the local launches use must stay inside this rank's temp slab.
+        const uint64_t slab_end = (uint64_t)base + rsize[la] * d.buffer_stride[la - 1];
+        auto local = [&](uint32_t a, bool barrier) -> int {
+            const uint64_t t0 = g.temp_elems;
+            const size_t at = list.size();
+            g.temp_elems = 0;
+            int r = a == 0 ? (fused ? axis0(!inv, inv ? norm : 1.0) : axis0_composed(!inv, inv ? norm : 1.0))
+                           : plan_c2c_axis(g, list, lcsize, a, inv, buf, buf, 1.0, 0);
+            if (r == R_SUCCESS && g.temp_elems > slab_end) r = R_UNSUPPORTED_FFT_LENGTH;
+            g.temp_elems = std::max(t0, g.temp_elems);
+            if (r == R_SUCCESS && barrier && list.size() > at) list[at].sync_before = true;
+            count(a);
+            return r;
+        };
+        if (!inv) {
+            for (uint32_t a = 0; a < la; ++a)
+                if ((a == 0 || d.size[a] > 1) && (rc = local(a, false)) != R_SUCCESS) return rc;
+            if ((rc = plan_c2c_axis(g, list, csize, la, 0, buf, buf, 1.0, 1, true)) != R_SUCCESS) return rc;
+            count(la);
+        } else {
+            if ((rc = plan_c2c_axis(g, list, csize, la, 1, buf, buf, 1.0, 1, true)) != R_SUCCESS) return rc;
+            count(la);
+            bool barrier = true;
+            for (uint32_t a = la; a-- > 0;) {
+                if (a > 0 && d.size[a] == 1) continue;
+                if ((rc = local(a, barrier)) != R_SUCCESS) return rc;
+                barrier = false;
+            }
+        }
+        return R_SUCCESS;
+    }
     if (!inv) {
         if ((rc = axis0_any(true, 1.0)) != R_SUCCESS) return rc;
         count(0);
@@ -1618,13 +1686,23 @@ static int build_plan_impl(const b200fft_desc& din, PlanGraph& g) {
         fill(d.buffer_stride, d.size[0]); fill(d.input_stride, d.size[0]); fill(d.output_stride, d.size[0]);
     }
     if (d.dist_world > 1) {
-        // one long in-place C2C sequence over peer windows: nothing else is defined for a distributed plan
+        // in-place transforms over peer windows, one batch: nothing else is defined for a distributed plan
         if (d.dist_rank >= d.dist_world) return R_INVALID_DEVICE;
         // 1-D: one long sequence (Four-Step over the window).  2-D / 3-D: slabs along the last dimension, default strides.
-        if (d.fft_dim > 3 || d.number_batches * d.coordinate_features != 1 || d.perform_r2c || d.perform_dct || d.perform_dst ||
-            d.is_input_formatted || d.is_output_formatted || d.buffer_stride[0] != d.size[0] || d.omit_dimension[0])
+        // 2-D / 3-D R2C: slabs of the in-place layout (H = nx/2+1 complex per row), pitches that may be padded; even nx > 2
+        // only, whose x axis needs no scratch beyond the rank's own slab (the odd lengths' composed path does)
+        const bool r2c_slab = d.perform_r2c && (d.fft_dim == 2 || d.fft_dim == 3);
+        if (d.fft_dim > 3 || d.number_batches * d.coordinate_features != 1 || (d.perform_r2c && !r2c_slab) || d.perform_dct ||
+            d.perform_dst || d.is_input_formatted || d.is_output_formatted || d.omit_dimension[0] ||
+            (!r2c_slab && d.buffer_stride[0] != d.size[0]))
             return R_UNSUPPORTED_FFT_LENGTH;
-        if (d.fft_dim > 1) {
+        if (r2c_slab) {
+            for (uint32_t a = 0; a < d.fft_dim; ++a)
+                if (d.omit_dimension[a]) return R_UNSUPPORTED_FFT_LENGTH;
+            if (d.size[0] % 2 || d.size[0] <= 2 || d.size[d.fft_dim - 1] % d.dist_world || d.buffer_stride[0] < d.size[0] / 2 + 1 ||
+                (d.fft_dim == 3 && d.buffer_stride[1] < d.size[1] * d.buffer_stride[0]))
+                return R_UNSUPPORTED_FFT_LENGTH;
+        } else if (d.fft_dim > 1) {
             uint64_t st = 1;
             for (uint32_t a = 0; a < d.fft_dim; ++a) {
                 st *= d.size[a];

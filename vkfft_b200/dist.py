@@ -171,25 +171,28 @@ class FusedDistributedFFT1D:
     def __init__(self, n, dist, device, double=False, normalize=False):
         import torch
         from . import api
-        from .window import PeerWindow
         self.torch, self.dist, self.api = torch, dist, api
         self.R, self.r = dist.get_world_size(), dist.get_rank()
         if n % self.R:
             raise ValueError("world size must divide N")
         esz = 16 if double else 8
         self.n = n
-        self.seq = PeerWindow(n // self.R * esz, dist, device)
-        self.tmp = PeerWindow(n // self.R * esz, dist, device)
-        dt = torch.complex128 if double else torch.complex64
-        self.local = self.seq.tensor(torch, dt)
         cfg = api.VkFFTConfiguration(FFTdim=1, size=[n], device=device, doublePrecision=int(double), normalize=int(normalize),
                                      userTempBuffer=1, distWorld=self.R, distRank=self.r)
-        self.app = api.VkFFTApplication()
-        rc = api.initializeVkFFT(self.app, cfg)
+        self._open(n // self.R * esz, cfg, device)
+        self.local = self.seq.tensor(torch, torch.complex128 if double else torch.complex64)
+
+    def _open(self, slab_bytes, cfg, device):
+        """the two peer windows (data and scratch, `slab_bytes` per rank) and this rank's plan, bound to the data window"""
+        from . import _lib
+        from .window import PeerWindow
+        self.seq = PeerWindow(slab_bytes, self.dist, device)
+        self.tmp = PeerWindow(slab_bytes, self.dist, device)
+        self.app = self.api.VkFFTApplication()
+        rc = self.api.initializeVkFFT(self.app, cfg)
         if rc != 0:
             self.close()
-            raise RuntimeError(api.getVkFFTErrorString(rc))
-        from . import _lib
+            raise RuntimeError(self.api.getVkFFTErrorString(rc))
         _lib.load().b200fft_plan_attach_window(self.app._plan, self.seq.handle)
 
     def __call__(self, inverse=False):
@@ -244,8 +247,7 @@ class FusedDistributedFFTND(FusedDistributedFFT1D):
 
     def __init__(self, shape_xyz, dist, device, double=False, normalize=False):
         import torch
-        from . import api, _lib
-        from .window import PeerWindow
+        from . import api
         self.torch, self.dist, self.api = torch, dist, api
         self.R, self.r = dist.get_world_size(), dist.get_rank()
         shape_xyz = tuple(int(v) for v in shape_xyz)
@@ -259,17 +261,76 @@ class FusedDistributedFFTND(FusedDistributedFFT1D):
         esz = 16 if double else 8
         self.n = total
         self.shape_xyz = shape_xyz
-        self.seq = PeerWindow(total // self.R * esz, dist, device)
-        self.tmp = PeerWindow(total // self.R * esz, dist, device)
+        cfg = api.VkFFTConfiguration(FFTdim=len(shape_xyz), size=list(shape_xyz), device=device, doublePrecision=int(double),
+                                     normalize=int(normalize), userTempBuffer=1, distWorld=self.R, distRank=self.r)
+        self._open(total // self.R * esz, cfg, device)
         dt = torch.complex128 if double else torch.complex64
         local_shape = (shape_xyz[-1] // self.R,) + tuple(reversed(shape_xyz[:-1]))
         self.local = self.seq.tensor(torch, dt).reshape(local_shape)
-        cfg = api.VkFFTConfiguration(FFTdim=len(shape_xyz), size=list(shape_xyz), device=device, doublePrecision=int(double),
-                                     normalize=int(normalize), userTempBuffer=1, distWorld=self.R, distRank=self.r)
-        self.app = api.VkFFTApplication()
-        rc = api.initializeVkFFT(self.app, cfg)
-        if rc != 0:
-            self.close()
-            raise RuntimeError(api.getVkFFTErrorString(rc))
-        _lib.load().b200fft_plan_attach_window(self.app._plan, self.seq.handle)
+
+
+def r2c_slab_pitches(shape_xyz, world, esz, granularity):
+    """complex-element pitches (bufferStride) of the in-place R2C layout whose slabs -- n_last/world outermost indices each --
+    fill whole mapping granules: H = nx/2+1 complex per row, and only the outermost pitch of a slab (the row pitch in 2-D, the
+    plane pitch in 3-D) padded, to the smallest value that makes a slab a multiple of `granularity` bytes.  Whenever n_last/world
+    is a power of two that adds less than one granule per slab."""
+    import math
+    nx, rows = shape_xyz[0], shape_xyz[-1] // world
+    h = nx // 2 + 1
+    inner = h if len(shape_xyz) == 2 else h * shape_xyz[1]
+    step = granularity // math.gcd(granularity, rows * esz)       # pitch multiple that makes rows * pitch * esz whole granules
+    outer = -(-inner // step) * step
+    return [outer, outer * shape_xyz[1]] if len(shape_xyz) == 2 else [h, outer, outer * shape_xyz[2]]
+
+
+class FusedDistributedRFFTND(FusedDistributedFFT1D):
+    """A 2-D or 3-D real-to-complex transform (and its complex-to-real inverse) whose array is spread over the GPUs of a box in
+    slabs along its last dimension, like FusedDistributedFFTND, in the in-place R2C layout.
+
+    `shape_xyz` = (nx, ny[, nz]) with x fastest, nx even.  Every row holds H = nx/2+1 complex points (the spectrum) or, before the
+    forward transform and after the inverse one, nx reals in the same memory.  Rank g holds the last-dimension indices
+    [g*n/R, (g+1)*n/R).  Its slab is padded on its outermost pitch only (`pitches`, complex elements: r2c_slab_pitches) so that it
+    maps onto whole granules of the peer window.  Two views of the same memory:
+
+        local   complex spectrum of shape (n/R, [ny,] H)
+        real    the real field, shape (n/R, [ny,] nx), row pitch 2*pitches[0] reals
+
+    `self()` runs the R2C forward, `self(inverse=True)` the C2R inverse (scaled by 1/(nx*ny[*nz]) with `normalize`), in place and
+    asynchronously on the current stream.  Forward: x (and y) inside the slab, a device-side barrier, the last axis across the
+    slabs on this rank's share of the spectrum columns; the inverse the other way round."""
+
+    def __init__(self, shape_xyz, dist, device, double=False, normalize=False):
+        import torch
+        from . import api, _lib
+        self.torch, self.dist, self.api = torch, dist, api
+        self.R, self.r = dist.get_world_size(), dist.get_rank()
+        shape_xyz = tuple(int(v) for v in shape_xyz)
+        if not 2 <= len(shape_xyz) <= 3:
+            raise ValueError("2-D or 3-D shapes")
+        if shape_xyz[0] % 2 or shape_xyz[0] <= 2:
+            raise ValueError("nx must be even and larger than 2")
+        if shape_xyz[-1] % self.R:
+            raise ValueError("world size must divide the last dimension")
+        esz = 16 if double else 8
+        gran = int(_lib.load().b200fft_window_granularity(int(device)))
+        if gran == 0:
+            raise RuntimeError("CUDA virtual memory management is not available on this device")
+        self.shape_xyz = shape_xyz
+        self.pitches = r2c_slab_pitches(shape_xyz, self.R, esz, gran)
+        rows = shape_xyz[-1] // self.R
+        nd = len(shape_xyz)
+        self.n = 1
+        for v in shape_xyz:
+            self.n *= v
+        cfg = api.VkFFTConfiguration(FFTdim=nd, size=list(shape_xyz), performR2C=1, bufferStride=list(self.pitches), device=device,
+                                     doublePrecision=int(double), normalize=int(normalize), userTempBuffer=1,
+                                     distWorld=self.R, distRank=self.r)
+        self._open(rows * self.pitches[nd - 2] * esz, cfg, device)
+        h = shape_xyz[0] // 2 + 1
+        inner = tuple(reversed(shape_xyz[1:-1]))                          # (ny,) in 3-D
+        inner_pitch = tuple(self.pitches[:nd - 2][::-1])                  # (H,) in 3-D
+        cdt, rdt = (torch.complex128, torch.float64) if double else (torch.complex64, torch.float32)
+        self.local = self.seq.tensor(torch, cdt).as_strided((rows,) + inner + (h,), (self.pitches[nd - 2],) + inner_pitch + (1,))
+        self.real = self.seq.tensor(torch, rdt).as_strided((rows,) + inner + (shape_xyz[0],),
+                                                           tuple(2 * p for p in (self.pitches[nd - 2],) + inner_pitch) + (1,))
 
