@@ -27,7 +27,8 @@ enum {
                              // post-pass on store (n+1 outputs), inverse: Hermitian pre-pass on load (n+1 inputs); aux0 = e^{-2 pi i k/2n}
     B2_OP_DCT23 = 32,        // specialised kernels: DCT-II (forward FFT: Makhoul gather on load, split + phase on store) or
                              // DCT-III (inverse FFT: phase + merge on load, Makhoul scatter on store); aux0 = e^{-i pi k/2n},
-                             // aux_u0 = number of real lines, aux_u1 = pitch between the two real lines of a pair
+                             // aux_u0 = number of real lines.  Contiguous lines: a complex line is a pair of real lines, aux_u1 =
+                             // their distance on the load side, aux_u2 on the store side (out of place the pitches differ)
     B2_OP_PERM_IN = 64,      // strided Four-Step first launch of a long DCT-II: rows are gathered through the Makhoul
                              // permutation of the FULL index p*N2 + n2 (aux_u0 = full length, aux_u1 = N2, n2 = coordinate tw_sel)
     B2_OP_BLUESTEIN = 256,   // specialised kernels: Bluestein launches on contiguous lines.  Forward kernel = first launch (zero-pad to n,
@@ -106,6 +107,7 @@ typedef struct b2_pass_params {
     uint32_t tw_sel;                       // which coordinate is the four-step "line": 0 group index, 1..3 outer dim 0..2
     uint32_t dst_flags;                    // B2_DST_* wrappers around the DCT operators
     uint32_t gen_flags;                    // B2_GEN_*: first stage reads its legs from HBM / last stage writes its outputs to HBM
+    uint32_t aux_u2;                       // operator specific (B2_OP_DCT23 on contiguous lines: pair distance on the store side)
 } b2_pass_params;
 
 enum {

@@ -142,7 +142,7 @@ struct PassReq {
     int inner_inverse = 0;
     uint32_t in_len = 0, out_len = 0;   // 0 -> n
     int aux0 = -1, aux1 = -1;
-    uint32_t aux_u0 = 0, aux_u1 = 0;
+    uint32_t aux_u0 = 0, aux_u1 = 0, aux_u2 = 0;
     bool real_pairs = false;     // group dim counts REAL lines; two of them form one complex line
     uint32_t dst_flags = 0;
     bool scalar_units = false;   // specialised real-data kernels addressing real lines: offsets/strides count scalars
@@ -282,7 +282,7 @@ int emit(PlanGraph& g, std::vector<PassPlan>& list, const PassReq& rq) {
         P.in_len = rq.in_len ? rq.in_len : rq.n;
         P.out_len = rq.out_len ? rq.out_len : rq.n;
         P.load_qfast = qfast_l; P.store_qfast = qfast_s;
-        P.aux_u0 = rq.aux_u0; P.aux_u1 = rq.aux_u1;
+        P.aux_u0 = rq.aux_u0; P.aux_u1 = rq.aux_u1; P.aux_u2 = rq.aux_u2;
         P.dst_flags = rq.dst_flags;
         pp.in_role = rq.in_role; pp.out_role = rq.out_role;
         pp.in_off = ioff + rq.in_base; pp.out_off = ooff + rq.out_base;
@@ -1416,7 +1416,6 @@ int plan_direction_r2c(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
 // for DCT-IV which maps one real line of length N to one complex line of length N/2.
 int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
     const b200fft_desc& d = g.desc;
-    if (d.is_input_formatted || d.is_output_formatted) return R_UNSUPPORTED_FFT_LENGTH_R2R;
     const bool is_dst = d.perform_dst != 0;
     int type = (int)(is_dst ? d.perform_dst : d.perform_dct);
     if (inv && (type == 2 || type == 3)) type = 5 - type;
@@ -1424,7 +1423,11 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
     for (uint32_t a = 0; a < d.fft_dim; ++a)
         if (!d.omit_dimension[a] && d.size[a] > 1) axes.push_back(a);
     if (inv) std::reverse(axes.begin(), axes.end());
+    // out of place: the same data flow as plan_direction_c2c -- the first axis reads the formatted source, the last axis
+    // writes the formatted destination, everything in between lives in `buffer`.  No launch writes the source.
     const Layout buf = layout_of(ROLE_BUFFER, d.buffer_stride, d.fft_dim);
+    const Layout inl = layout_of(ROLE_INPUT, d.input_stride, d.fft_dim);
+    const Layout outl = layout_of(ROLE_OUTPUT, d.output_stride, d.fft_dim);
     size_t dct_mark = list.size();
     uint32_t dct_prev_axis = ~0u;
     for (size_t i = 0; i <= axes.size(); ++i) {
@@ -1434,6 +1437,14 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
         const uint32_t axis = axes[i];
         dct_prev_axis = axis;
         const uint64_t N = d.size[axis];
+        Layout in = buf, out = buf;
+        if (!inv) {
+            if (i == 0 && d.is_input_formatted) in = inl;
+            if (i + 1 == axes.size() && d.is_output_formatted) out = outl;
+        } else {
+            if (i == 0 && d.is_output_formatted) in = outl;
+            if (i + 1 == axes.size() && d.is_input_formatted && d.inverse_return_to_input) out = inl;
+        }
         double scale = 1.0;
         if (inv && d.normalize) scale = 1.0 / (type == 1 ? (is_dst ? 2.0 * (double)(N + 1) : 2.0 * (double)(N - 1)) : 2.0 * (double)N);
         uint64_t n;
@@ -1461,25 +1472,32 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
         if (!is_dst && (type == 2 || type == 3)) {
             const int kkind = axis == 0 ? B2_KIND_ROWS : B2_KIND_COLS;
             const int kinv = type == 3 ? 1 : 0;
-            std::vector<Dim> lines = other_dims(g, d.size, axis, buf, buf);
+            std::vector<Dim> lines = other_dims(g, d.size, axis, in, out);
             bool ok = b2_find_kernel(kkind, g.prec, (int)N, kinv, B2_OP_DCT23) != nullptr;
             PassReq fr;
             fr.kind = kkind; fr.n = (int)N; fr.inv = kinv; fr.ops = B2_OP_DCT23 | ((scale != 1.0) ? B2_OP_SCALE : 0);
             fr.scale = scale; fr.aux0 = aux_for(g, AUX_DCT23, N);
+            fr.in_role = in.role; fr.out_role = out.role;
             fr.what = "dct axis (fused)";
+            // complex view of the real data (pairs of neighbouring columns): size[0] and every stride of both sides even
+            auto even_view = [&](const Layout& l) {
+                bool e = l.batch_stride % 2 == 0;
+                for (uint32_t a = 1; a < d.fft_dim; ++a) e = e && (l.stride[a - 1] % 2 == 0);
+                return e;
+            };
+            const bool view_ok = axis != 0 && d.size[0] % 2 == 0 && even_view(in) && even_view(out);
             if (ok && axis == 0) {
+                // the kernel pairs real lines 2j and 2j+1 of the group: aux_u1 / aux_u2 = their distance on the load / store side
                 std::vector<Dim> m = merge_dims(lines);
                 Dim grp = m.empty() ? Dim{1, 0, 0} : m[0];
                 if (!m.empty()) m.erase(m.begin());
                 fr.real_pairs = true; fr.scalar_units = true;
-                fr.aux_u0 = (uint32_t)grp.n; fr.aux_u1 = (uint32_t)grp.is;
+                fr.aux_u0 = (uint32_t)grp.n; fr.aux_u1 = (uint32_t)grp.is; fr.aux_u2 = (uint32_t)grp.os;
                 fr.group = Dim{grp.n, 2 * grp.is, 2 * grp.os};
                 fr.outer = m;
                 fr.in_es = fr.out_es = 1;
             } else if (ok) {
-                // complex view: size[0] and every stride must be even
-                ok = (d.size[0] % 2 == 0) && (buf.stride[axis - 1] % 2 == 0) && (buf.batch_stride % 2 == 0);
-                for (uint32_t a = 1; a < d.fft_dim && ok; ++a) ok = (buf.stride[a - 1] % 2 == 0);
+                ok = view_ok;
                 if (ok) {
                     std::vector<Dim> cl;
                     cl.push_back(Dim{d.size[0] / 2, 1, 1});
@@ -1488,18 +1506,17 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
                     if (!m.empty() && m[0].is == 1) { fr.group = m[0]; m.erase(m.begin()); }
                     else fr.group = Dim{1, 1, 1};
                     fr.outer = m;
-                    fr.in_es = fr.out_es = (int64_t)buf.stride[axis - 1] / 2;
+                    fr.in_es = (int64_t)in.stride[axis - 1] / 2;
+                    fr.out_es = (int64_t)out.stride[axis - 1] / 2;
                 }
             }
             // long strided axis (no well-shaped single-launch kernel): Four-Step along the stride with the Makhoul
             // permutation folded into the first gather (DCT-II) / the last scatter (DCT-III) and a separate split/merge launch
             bool long_strided = false;
             uint64_t L1 = 0, L2 = 0;
-            if (axis != 0 && (d.size[0] % 2 == 0) && N % 2 == 0) {
+            if (view_ok && N % 2 == 0) {
                 const b2_kernel_info* single = b2_find_kernel(B2_KIND_COLS, g.prec, (int)N, kinv, B2_OP_DCT23);
-                bool strides_even = (buf.batch_stride % 2 == 0);
-                for (uint32_t a = 1; a < d.fft_dim; ++a) strides_even = strides_even && (buf.stride[a - 1] % 2 == 0);
-                if (strides_even && (!single || single->q < 8)) {
+                if (!single || single->q < 8) {
                     uint64_t bestc = ~0ull;
                     for (uint64_t n2 = 2; n2 * 2 <= N; ++n2) {
                         if (N % n2) continue;
@@ -1515,38 +1532,41 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
                 }
             }
             if (long_strided) {
-                const int64_t esc = (int64_t)buf.stride[axis - 1] / 2;
+                // scratch and every launch after the first one use the destination's complex view (esc, rest[].os):
+                // DCT-II   source -> temp (gather+phase), temp -> destination, split+phase in place on the destination;
+                // DCT-III  source -> destination (phase+merge), destination -> temp, temp -> destination (scatter)
+                const int64_t esc_in = (int64_t)in.stride[axis - 1] / 2, esc = (int64_t)out.stride[axis - 1] / 2;
                 std::vector<Dim> cl;   // complex-view line dims: columns first
                 cl.push_back(Dim{d.size[0] / 2, 1, 1});
                 for (size_t li = 1; li < lines.size(); ++li) cl.push_back(Dim{lines[li].n, lines[li].is / 2, lines[li].os / 2});
                 std::vector<Dim> m = merge_dims(cl);
                 if (m.empty() || m[0].is != 1) return R_UNSUPPORTED_FFT_LENGTH_R2R;
                 const Dim unit = m[0];
-                std::vector<Dim> rest(m.begin() + 1, m.end());
+                std::vector<Dim> rest(m.begin() + 1, m.end()), rest_out;
+                for (const Dim& dd : rest) rest_out.push_back(Dim{dd.n, dd.os, dd.os});
                 uint64_t extent = (uint64_t)esc * N;
                 for (const Dim& dd : cl) extent = std::max<uint64_t>(extent, (uint64_t)dd.n * (uint64_t)dd.os);
                 g.temp_elems = std::max<uint64_t>(g.temp_elems, extent);
                 const int aux = aux_for(g, AUX_DCT23, N);
                 PassReq ew;
                 ew.elementwise = true; ew.n = (int)unit.n; ew.ew_items = (uint32_t)unit.n;
-                ew.in_es = ew.out_es = 1; ew.in_role = ew.out_role = ROLE_BUFFER;
+                ew.in_es = ew.out_es = 1; ew.out_role = out.role;
                 ew.aux0 = aux; ew.aux_u0 = (uint32_t)N;
                 std::vector<Dim> ewl;
-                ewl.push_back(Dim{N / 2 + 1, esc, esc});
-                for (const Dim& dd : rest) ewl.push_back(dd);
                 int rcl;
                 PassReq a, b;
                 a.kind = b.kind = B2_KIND_COLS; a.n = (int)L1; b.n = (int)L2; a.inv = b.inv = kinv;
                 a.group = unit; b.group = Dim{unit.n, 1, 1};
-                a.in_es = a.out_es = esc * (int64_t)L2;
+                const int64_t esa = kinv == 0 ? esc_in : esc;   // DCT-II: pass A reads the source, DCT-III: the destination
+                a.in_es = esa * (int64_t)L2; a.out_es = esc * (int64_t)L2;
                 a.outer.push_back(Dim{L2, kinv == 0 ? 0 : esc, esc});
                 a.tw_outer = 0; a.twM = N;
-                for (const Dim& dd : rest) a.outer.push_back(dd);
-                a.in_role = ROLE_BUFFER; a.out_role = ROLE_TEMP;
+                for (const Dim& dd : (kinv == 0 ? rest : rest_out)) a.outer.push_back(dd);
+                a.in_role = kinv == 0 ? in.role : out.role; a.out_role = ROLE_TEMP;
                 b.in_es = esc; b.out_es = esc * (int64_t)L1;
                 b.outer.push_back(Dim{L1, esc * (int64_t)L2, kinv == 0 ? esc : 0});
-                for (const Dim& dd : rest) b.outer.push_back(dd);
-                b.in_role = ROLE_TEMP; b.out_role = ROLE_BUFFER;
+                for (const Dim& dd : rest_out) b.outer.push_back(dd);
+                b.in_role = ROLE_TEMP; b.out_role = out.role;
                 if (kinv == 0) {   // DCT-II
                     a.ops = B2_OP_TWIDDLE_OUT | B2_OP_PERM_IN; a.aux_u0 = (uint32_t)N; a.aux_u1 = (uint32_t)L2;
                     a.what = "long dct-ii 1/3 gather+phase";
@@ -1554,9 +1574,15 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
                     b.ops = 0; b.what = "long dct-ii 2/3";
                     if ((rcl = emit(g, list, b)) != R_SUCCESS) return rcl;
                     ew.ew_op = 3; ew.ops = (scale != 1.0) ? B2_OP_SCALE : 0; ew.scale = scale; ew.what = "long dct-ii 3/3 split+phase";
+                    ew.in_role = out.role;
+                    ewl.push_back(Dim{N / 2 + 1, esc, esc});
+                    ewl.insert(ewl.end(), rest_out.begin(), rest_out.end());
                     if ((rcl = emit_ew(g, list, ew, ewl)) != R_SUCCESS) return rcl;
                 } else {           // DCT-III
                     ew.ew_op = 4; ew.what = "long dct-iii 1/3 phase+merge";
+                    ew.in_role = in.role;
+                    ewl.push_back(Dim{N / 2 + 1, esc_in, esc});
+                    ewl.insert(ewl.end(), rest.begin(), rest.end());
                     if ((rcl = emit_ew(g, list, ew, ewl)) != R_SUCCESS) return rcl;
                     a.ops = B2_OP_TWIDDLE_OUT; a.what = "long dct-iii 2/3";
                     if ((rcl = emit(g, list, a)) != R_SUCCESS) return rcl;
@@ -1588,8 +1614,8 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
                 default: io = B2_IO_DCT4_ODD; nc = 2 * N; a0 = aux_for(g, AUX_DCT4ODD_PRE, N); a1 = aux_for(g, AUX_DCT4ODD_POST, N); break;
             }
             if (nc > 0x7fffffffull) return R_UNSUPPORTED_FFT_LENGTH_R2R;
-            const int64_t es_r = axis == 0 ? 1 : (int64_t)buf.stride[axis - 1];
-            std::vector<Dim> real_lines = other_dims(g, d.size, axis, buf, buf), r2t, t2t, t2r;
+            const int64_t es_in = axis == 0 ? 1 : (int64_t)in.stride[axis - 1], es_out = axis == 0 ? 1 : (int64_t)out.stride[axis - 1];
+            std::vector<Dim> real_lines = other_dims(g, d.size, axis, in, out), r2t, t2t, t2r;
             uint64_t ts = nc, nlines = 1;
             for (const Dim& rl : real_lines) {
                 r2t.push_back(Dim{rl.n, rl.is, (int64_t)ts});
@@ -1602,8 +1628,8 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
             PassReq ew;
             ew.elementwise = true; ew.store_io = io; ew.dst_flags = dflags; ew.aux0 = a0; ew.aux1 = a1;
             ew.aux_u0 = (uint32_t)N; ew.aux_u1 = (uint32_t)nc;
-            ew.ew_op = 9; ew.n = (int)nc; ew.ew_items = (uint32_t)nc; ew.in_es = es_r; ew.out_es = 1;
-            ew.in_role = ROLE_BUFFER; ew.out_role = ROLE_TEMP; ew.what = "r2r (composed): operator load side";
+            ew.ew_op = 9; ew.n = (int)nc; ew.ew_items = (uint32_t)nc; ew.in_es = es_in; ew.out_es = 1;
+            ew.in_role = in.role; ew.out_role = ROLE_TEMP; ew.what = "r2r (composed): operator load side";
             int rc2;
             if ((rc2 = emit_ew(g, list, ew, r2t)) != R_SUCCESS) return rc2;
             list.back().in_scalar = true;
@@ -1612,8 +1638,8 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
             job.in_role = job.out_role = ROLE_TEMP; job.tmp_base = (int64_t)region; job.scale = 1.0;
             if ((rc2 = plan_c2c(g, list, job)) != R_SUCCESS) return rc2 == R_UNSUPPORTED_FFT_LENGTH ? R_UNSUPPORTED_FFT_LENGTH_R2R : rc2;
             const uint64_t items = (type == 3) ? nc : N;
-            ew.ew_op = 10; ew.n = (int)items; ew.ew_items = (uint32_t)items; ew.in_es = 1; ew.out_es = es_r;
-            ew.in_role = ROLE_TEMP; ew.out_role = ROLE_BUFFER; ew.what = "r2r (composed): operator store side";
+            ew.ew_op = 10; ew.n = (int)items; ew.ew_items = (uint32_t)items; ew.in_es = 1; ew.out_es = es_out;
+            ew.in_role = ROLE_TEMP; ew.out_role = out.role; ew.what = "r2r (composed): operator store side";
             ew.ops = (scale != 1.0) ? B2_OP_SCALE : 0; ew.scale = scale;
             if ((rc2 = emit_ew(g, list, ew, t2r)) != R_SUCCESS) return rc2;
             list.back().out_scalar = true;
@@ -1626,8 +1652,10 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
         }
         rq.n = (int)n;
         rq.kind = axis == 0 ? B2_KIND_ROWS : B2_KIND_COLS;
-        rq.in_es = rq.out_es = axis == 0 ? 1 : (int64_t)buf.stride[axis - 1];
-        std::vector<Dim> lines = other_dims(g, d.size, axis, buf, buf);
+        rq.in_es = axis == 0 ? 1 : (int64_t)in.stride[axis - 1];
+        rq.out_es = axis == 0 ? 1 : (int64_t)out.stride[axis - 1];
+        rq.in_role = in.role; rq.out_role = out.role;
+        std::vector<Dim> lines = other_dims(g, d.size, axis, in, out);
         std::vector<Dim> m = merge_dims(lines);
         if (axis != 0) {
             if (!m.empty() && m[0].is == 1) { rq.group = m[0]; m.erase(m.begin()); }

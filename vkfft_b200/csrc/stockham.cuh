@@ -494,7 +494,7 @@ struct Engine {
         bool vb = false;
         if constexpr (C::LAYOUT == LAY_LINE) {
             oa = (T*)P.out + obase_out + (int64_t)gl * P.out_gs;
-            ob = oa + P.aux_u1;
+            ob = oa + P.aux_u2;
             vb = (2 * gl + 1 < P.aux_u0);
         } else {
             oc = (X*)P.out + obase_out + (int64_t)gl * P.out_gs;

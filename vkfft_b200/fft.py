@@ -9,7 +9,7 @@ This module gives the same surface over the C ABI:
     vkfft.ifftn(y, y)                 # in place
     h = vkfft.rfftn(r, ndim=2)        # real -> half-Hermitian complex (last axis n//2+1)
     r2 = vkfft.irfftn(h, ndim=2, n_last=r.shape[-1])
-    c = vkfft.dctn(r, dct_type=2)     # FFTW REDFT10 convention, idctn / dstn / idstn likewise
+    c = vkfft.dctn(r, dct_type=2)     # FFTW REDFT10 convention, idctn / dstn / idstn likewise (out of place: r is not written)
 
 `ndim` = number of trailing dimensions to transform (the fast axes; leading dimensions are batches), as in pyvkfft.
 `norm`: 0 = nothing (the library's own convention: unnormalised inverse), 1 = backward transform scaled by 1/N (numpy's
@@ -226,17 +226,34 @@ def _r2r(src, dest, ndim, norm, cuda_stream, inverse, kind, dst):
     if src.is_complex():
         raise TypeError("real tensor expected")
     prec = _prec(src, {k: v for k, v in _REAL_PREC.items() if v != 2}, "dctn / dstn")    # no half cosine / sine transforms
+    inplace = dest is not None and dest.data_ptr() == src.data_ptr()
     if dest is None:
-        dest = src.clone()
-    elif dest.data_ptr() != src.data_ptr():
-        _check(dest, "dest")
-        dest.copy_(src)
+        dest = torch.empty_like(src)
+    _check(dest, "dest")
+    if dest.shape != src.shape or dest.dtype != src.dtype:
+        raise ValueError("dest must match src")
     nd, sizes, batch = _split(src.shape, ndim)
     dev = src.device.index
+    if all(s == 1 for s in sizes):
+        # no axis has a launch: the transform is the identity (as in _c2c)
+        if not inplace:
+            with torch.cuda.stream(torch.cuda.ExternalStream(_stream(torch, cuda_stream))):
+                dest.copy_(src)
+        return dest
+    # out of place as in _c2c: the forward transform reads inputBuffer, the inverse reads outputBuffer, the result is in
+    # `buffer`; the source is not written
+    fmt = {} if inplace else ({"isOutputFormatted": 1, "makeInversePlanOnly": 1} if inverse else
+                              {"isInputFormatted": 1, "makeForwardPlanOnly": 1})
     name = "performDST" if dst else "performDCT"
-    app = _plan((name, kind, tuple(sizes), batch, prec, dev), FFTdim=nd, size=sizes, numberBatches=batch, device=dev,
-                doublePrecision=int(prec == 1), **{name: kind})
-    rc = api.VkFFTAppend(app, 1 if inverse else -1, api.VkFFTLaunchParams(buffer=dest, stream=_stream(torch, cuda_stream)))
+    app = _plan((name, kind, tuple(sizes), batch, prec, dev, inplace, inverse and not inplace), FFTdim=nd, size=sizes,
+                numberBatches=batch, device=dev, doublePrecision=int(prec == 1), **{name: kind}, **fmt)
+    lp = api.VkFFTLaunchParams(buffer=dest, stream=_stream(torch, cuda_stream))
+    if not inplace:
+        if inverse:
+            lp.outputBuffer = src
+        else:
+            lp.inputBuffer = src
+    rc = api.VkFFTAppend(app, 1 if inverse else -1, lp)
     if rc != 0:
         raise RuntimeError("VkFFTAppend: " + api.getVkFFTErrorString(rc))
     n = 1
