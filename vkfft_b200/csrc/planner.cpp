@@ -463,6 +463,27 @@ bool slice_dim(Dim& d, uint32_t world, uint32_t rank, int64_t& in_base, int64_t&
     return true;
 }
 
+// distributed N-D plan, the axis that crosses the slabs: keep rank `rank`'s share of the line dimensions `lines` -- a contiguous
+// block of the outermost dimension with more than one line that `world` divides (never the batch entry, which is 1 here), or,
+// when none does and `ragged` is set, a range of lines[0] whose boundaries fall on multiples of 8 lines (neighbouring lanes of
+// one CTA), the last rank taking the remainder.  Moves the bases to the share's first line.
+int share_lines(std::vector<Dim>& lines, uint32_t world, uint32_t rank, bool ragged, int64_t& in_base, int64_t& out_base) {
+    for (size_t i = lines.size(); i-- > 0;) {
+        uint64_t first;
+        if (lines[i].n > 1 && lines[i].n % world == 0 && slice_dim(lines[i], world, rank, in_base, out_base, first)) return R_SUCCESS;
+    }
+    if (!ragged || lines.empty()) return R_UNSUPPORTED_FFT_LENGTH;
+    Dim& c = lines[0];
+    uint64_t per = c.n / world;
+    if (per >= 8) per &= ~7ull;
+    if (per == 0) return R_UNSUPPORTED_FFT_LENGTH;
+    const uint64_t first = (uint64_t)rank * per;
+    c.n = (rank + 1 == world) ? c.n - first : per;
+    in_base += (int64_t)first * c.is;
+    out_base += (int64_t)first * c.os;
+    return R_SUCCESS;
+}
+
 int plan_c2c(PlanGraph& g, std::vector<PassPlan>& list, const C2CJob& job);
 
 // elementwise helper launch over `lines` (every line dimension, any order)
@@ -785,24 +806,8 @@ int plan_c2c(PlanGraph& g, std::vector<PassPlan>& list, const C2CJob& job) {
     std::vector<Dim> sliced = job.lines;
     int64_t slice_in = 0, slice_out = 0;
     if (job.line_world > 1) {
-        // the outermost dimension with more than one line that divides evenly (never the batch entry, which is 1 here)
-        bool done = false;
-        for (size_t i = sliced.size(); i-- > 0 && !done;) {
-            uint64_t first;
-            if (sliced[i].n > 1 && sliced[i].n % job.line_world == 0) done = slice_dim(sliced[i], job.line_world, job.line_rank, slice_in, slice_out, first);
-        }
-        if (!done && job.line_ragged && !sliced.empty()) {
-            Dim& c = sliced[0];
-            uint64_t per = c.n / job.line_world;
-            if (per >= 8) per &= ~7ull;          // range boundaries on whole 8-column groups (neighbouring lanes of one CTA)
-            if (per == 0) return R_UNSUPPORTED_FFT_LENGTH;
-            const uint64_t first = (uint64_t)job.line_rank * per;
-            c.n = (job.line_rank + 1 == job.line_world) ? c.n - first : per;
-            slice_in += (int64_t)first * c.is;
-            slice_out += (int64_t)first * c.os;
-            done = true;
-        }
-        if (!done) return R_UNSUPPORTED_FFT_LENGTH;
+        const int rs = share_lines(sliced, job.line_world, job.line_rank, job.line_ragged, slice_in, slice_out);
+        if (rs != R_SUCCESS) return rs;
     }
     std::vector<Dim> m = merge_dims(sliced);
     const bool contiguous = (job.es_in == 1 && job.es_out == 1);
@@ -1070,11 +1075,27 @@ std::vector<Dim> other_dims(const PlanGraph& g, const uint64_t* size, uint32_t a
 
 // distributed N-D plan: first element of this rank's slab in `buffer` and in scratch (both windows have the same slabs).
 // Rank g owns indices [g*n/R, (g+1)*n/R) of the last dimension, so its slab starts g*n/R outermost pitches in -- for R2C
-// the pitches of the complex rows, which may be padded so that a slab fills whole mapping granules
+// the pitches of the complex rows, for DCT / DST those of the real rows (real elements); either may be padded so that a slab
+// fills whole mapping granules
 int64_t slab_base(const PlanGraph& g) {
     const b200fft_desc& d = g.desc;
     const uint32_t la = d.fft_dim - 1;
     return (int64_t)((uint64_t)d.dist_rank * (d.size[la] / d.dist_world) * d.buffer_stride[la - 1]);
+}
+
+// distributed N-D plan: one axis of the segment that stays inside this rank's slab, planned by `plan_axis`.  Its scratch must end
+// at or before `slab_end` (temp elements), the end of the rank's temp slab: a route that needs more is refused.  `barrier`:
+// the segment's first launch waits for every rank.
+template <class F>
+int plan_in_slab(PlanGraph& g, std::vector<PassPlan>& list, uint64_t slab_end, bool barrier, F&& plan_axis) {
+    const uint64_t t0 = g.temp_elems;
+    const size_t at = list.size();
+    g.temp_elems = 0;
+    int r = plan_axis();
+    if (r == R_SUCCESS && g.temp_elems > slab_end) r = R_UNSUPPORTED_FFT_LENGTH;
+    g.temp_elems = std::max(t0, g.temp_elems);
+    if (r == R_SUCCESS && barrier && list.size() > at) list[at].sync_before = true;
+    return r;
 }
 
 // slab: < 0 ordinary plan;  0: local axis of a distributed N-D plan (this rank's slab only: `size` already holds the slab's
@@ -1362,14 +1383,10 @@ int plan_direction_r2c(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
         // runs the other way round.  Whatever scratch the local launches use must stay inside this rank's temp slab.
         const uint64_t slab_end = (uint64_t)base + rsize[la] * d.buffer_stride[la - 1];
         auto local = [&](uint32_t a, bool barrier) -> int {
-            const uint64_t t0 = g.temp_elems;
-            const size_t at = list.size();
-            g.temp_elems = 0;
-            int r = a == 0 ? (fused ? axis0(!inv, inv ? norm : 1.0) : axis0_composed(!inv, inv ? norm : 1.0))
-                           : plan_c2c_axis(g, list, lcsize, a, inv, buf, buf, 1.0, 0);
-            if (r == R_SUCCESS && g.temp_elems > slab_end) r = R_UNSUPPORTED_FFT_LENGTH;
-            g.temp_elems = std::max(t0, g.temp_elems);
-            if (r == R_SUCCESS && barrier && list.size() > at) list[at].sync_before = true;
+            const int r = plan_in_slab(g, list, slab_end, barrier, [&] {
+                return a == 0 ? (fused ? axis0(!inv, inv ? norm : 1.0) : axis0_composed(!inv, inv ? norm : 1.0))
+                              : plan_c2c_axis(g, list, lcsize, a, inv, buf, buf, 1.0, 0);
+            });
             count(a);
             return r;
         };
@@ -1428,23 +1445,13 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
     const Layout buf = layout_of(ROLE_BUFFER, d.buffer_stride, d.fft_dim);
     const Layout inl = layout_of(ROLE_INPUT, d.input_stride, d.fft_dim);
     const Layout outl = layout_of(ROLE_OUTPUT, d.output_stride, d.fft_dim);
-    size_t dct_mark = list.size();
-    uint32_t dct_prev_axis = ~0u;
-    for (size_t i = 0; i <= axes.size(); ++i) {
-        if (dct_prev_axis != ~0u) g.axis_uploads[inv ? 1 : 0][dct_prev_axis] += (uint32_t)(list.size() - dct_mark);
-        dct_mark = list.size();
-        if (i == axes.size()) break;
-        const uint32_t axis = axes[i];
-        dct_prev_axis = axis;
-        const uint64_t N = d.size[axis];
-        Layout in = buf, out = buf;
-        if (!inv) {
-            if (i == 0 && d.is_input_formatted) in = inl;
-            if (i + 1 == axes.size() && d.is_output_formatted) out = outl;
-        } else {
-            if (i == 0 && d.is_output_formatted) in = outl;
-            if (i + 1 == axes.size() && d.is_input_formatted && d.inverse_return_to_input) out = inl;
-        }
+    // One axis.  `size`: the extents its lines are counted over.  Distributed plans (slabs along the last dimension): a local
+    // axis gets the slab's extents and `base`, the slab's first real element; the axis that crosses the slabs (`share`) runs on
+    // this rank's share of its lines (share_lines over column pairs: the complex view and the paired real lines of the
+    // runtime-scheduled kernel both read two neighbouring columns as one line, so a pair is never cut).
+    auto plan_axis = [&](uint32_t axis, const uint64_t* size, const Layout& in, const Layout& out, int64_t base, bool share) -> int {
+        const uint64_t N = size[axis];
+        const int64_t cbase = (base + 1) / 2;   // first element of the slab in complex units (scratch, complex view)
         double scale = 1.0;
         if (inv && d.normalize) scale = 1.0 / (type == 1 ? (is_dst ? 2.0 * (double)(N + 1) : 2.0 * (double)(N - 1)) : 2.0 * (double)N);
         uint64_t n;
@@ -1472,7 +1479,7 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
         if (!is_dst && (type == 2 || type == 3)) {
             const int kkind = axis == 0 ? B2_KIND_ROWS : B2_KIND_COLS;
             const int kinv = type == 3 ? 1 : 0;
-            std::vector<Dim> lines = other_dims(g, d.size, axis, in, out);
+            std::vector<Dim> lines = other_dims(g, size, axis, in, out);
             bool ok = b2_find_kernel(kkind, g.prec, (int)N, kinv, B2_OP_DCT23) != nullptr;
             PassReq fr;
             fr.kind = kkind; fr.n = (int)N; fr.inv = kinv; fr.ops = B2_OP_DCT23 | ((scale != 1.0) ? B2_OP_SCALE : 0);
@@ -1486,6 +1493,14 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
                 return e;
             };
             const bool view_ok = axis != 0 && d.size[0] % 2 == 0 && even_view(in) && even_view(out);
+            std::vector<Dim> cl, vl;              // complex-view line dims (columns first); vl: this rank's share of them
+            int64_t vin = cbase, vout = cbase;    // first complex element of vl on the load / store side
+            if (view_ok) {
+                cl.push_back(Dim{size[0] / 2, 1, 1});
+                for (size_t li = 1; li < lines.size(); ++li) cl.push_back(Dim{lines[li].n, lines[li].is / 2, lines[li].os / 2});
+                vl = cl;
+                if (share && share_lines(vl, d.dist_world, d.dist_rank, true, vin, vout) != R_SUCCESS) return R_UNSUPPORTED_FFT_LENGTH;
+            }
             if (ok && axis == 0) {
                 // the kernel pairs real lines 2j and 2j+1 of the group: aux_u1 / aux_u2 = their distance on the load / store side
                 std::vector<Dim> m = merge_dims(lines);
@@ -1496,18 +1511,17 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
                 fr.group = Dim{grp.n, 2 * grp.is, 2 * grp.os};
                 fr.outer = m;
                 fr.in_es = fr.out_es = 1;
+                fr.in_base = fr.out_base = base;
             } else if (ok) {
                 ok = view_ok;
                 if (ok) {
-                    std::vector<Dim> cl;
-                    cl.push_back(Dim{d.size[0] / 2, 1, 1});
-                    for (size_t li = 1; li < lines.size(); ++li) cl.push_back(Dim{lines[li].n, lines[li].is / 2, lines[li].os / 2});
-                    std::vector<Dim> m = merge_dims(cl);
+                    std::vector<Dim> m = merge_dims(vl);
                     if (!m.empty() && m[0].is == 1) { fr.group = m[0]; m.erase(m.begin()); }
                     else fr.group = Dim{1, 1, 1};
                     fr.outer = m;
                     fr.in_es = (int64_t)in.stride[axis - 1] / 2;
                     fr.out_es = (int64_t)out.stride[axis - 1] / 2;
+                    fr.in_base = vin; fr.out_base = vout;
                 }
             }
             // long strided axis (no well-shaped single-launch kernel): Four-Step along the stride with the Makhoul
@@ -1535,23 +1549,23 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
                 // scratch and every launch after the first one use the destination's complex view (esc, rest[].os):
                 // DCT-II   source -> temp (gather+phase), temp -> destination, split+phase in place on the destination;
                 // DCT-III  source -> destination (phase+merge), destination -> temp, temp -> destination (scatter)
+                // A rank's share of a distributed axis is whole columns (rows k and N-k of a column stay together): its three
+                // launches touch only its own columns in both windows and need no barrier between them.
                 const int64_t esc_in = (int64_t)in.stride[axis - 1] / 2, esc = (int64_t)out.stride[axis - 1] / 2;
-                std::vector<Dim> cl;   // complex-view line dims: columns first
-                cl.push_back(Dim{d.size[0] / 2, 1, 1});
-                for (size_t li = 1; li < lines.size(); ++li) cl.push_back(Dim{lines[li].n, lines[li].is / 2, lines[li].os / 2});
-                std::vector<Dim> m = merge_dims(cl);
+                std::vector<Dim> m = merge_dims(vl);
                 if (m.empty() || m[0].is != 1) return R_UNSUPPORTED_FFT_LENGTH_R2R;
                 const Dim unit = m[0];
                 std::vector<Dim> rest(m.begin() + 1, m.end()), rest_out;
                 for (const Dim& dd : rest) rest_out.push_back(Dim{dd.n, dd.os, dd.os});
                 uint64_t extent = (uint64_t)esc * N;
                 for (const Dim& dd : cl) extent = std::max<uint64_t>(extent, (uint64_t)dd.n * (uint64_t)dd.os);
-                g.temp_elems = std::max<uint64_t>(g.temp_elems, extent);
+                g.temp_elems = std::max<uint64_t>(g.temp_elems, (uint64_t)cbase + extent);
                 const int aux = aux_for(g, AUX_DCT23, N);
                 PassReq ew;
                 ew.elementwise = true; ew.n = (int)unit.n; ew.ew_items = (uint32_t)unit.n;
                 ew.in_es = ew.out_es = 1; ew.out_role = out.role;
                 ew.aux0 = aux; ew.aux_u0 = (uint32_t)N;
+                ew.in_base = kinv == 0 ? vout : vin; ew.out_base = vout;
                 std::vector<Dim> ewl;
                 int rcl;
                 PassReq a, b;
@@ -1563,6 +1577,7 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
                 a.tw_outer = 0; a.twM = N;
                 for (const Dim& dd : (kinv == 0 ? rest : rest_out)) a.outer.push_back(dd);
                 a.in_role = kinv == 0 ? in.role : out.role; a.out_role = ROLE_TEMP;
+                a.in_base = kinv == 0 ? vin : vout; a.out_base = b.in_base = b.out_base = vout;   // scratch at the data's positions
                 b.in_es = esc; b.out_es = esc * (int64_t)L1;
                 b.outer.push_back(Dim{L1, esc * (int64_t)L2, kinv == 0 ? esc : 0});
                 for (const Dim& dd : rest_out) b.outer.push_back(dd);
@@ -1591,19 +1606,17 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
                     b.what = "long dct-iii 3/3 scatter";
                     if ((rcl = emit(g, list, b)) != R_SUCCESS) return rcl;
                 }
-                continue;
+                return R_SUCCESS;
             }
-            if (ok) {
-                int rcf = emit(g, list, fr);
-                if (rcf != R_SUCCESS) return rcf;
-                continue;
-            }
+            if (ok) return emit(g, list, fr);
         }
         if (n < 2) return R_UNSUPPORTED_FFT_LENGTH_R2R;
         if (!is_smooth(n) || !generic_fits(g, n)) {
             // transform length with a prime factor above 127, or too long for one shared-memory pass: the operator's load
             // and store sides become launches of their own around an ordinary C2C plan on scratch (one real line per
-            // complex line; DCT-IV always in its zero-padded 2N form here)
+            // complex line; DCT-IV always in its zero-padded 2N form here).  A local axis of a distributed plan keeps the
+            // scratch in its temp slab (which it does not fit in practice); across the slabs the route is not planned.
+            if (share) return R_UNSUPPORTED_FFT_LENGTH;
             uint32_t dflags = 0;
             if (is_dst) dflags = type == 2 ? (B2_DST_NEG_ODD_IN | B2_DST_REV_OUT) : ((type == 3 || type == 4) ? (B2_DST_REV_IN | B2_DST_ALT_OUT) : 0);
             int io; uint64_t nc; int a0 = -1, a1 = -1;
@@ -1615,7 +1628,7 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
             }
             if (nc > 0x7fffffffull) return R_UNSUPPORTED_FFT_LENGTH_R2R;
             const int64_t es_in = axis == 0 ? 1 : (int64_t)in.stride[axis - 1], es_out = axis == 0 ? 1 : (int64_t)out.stride[axis - 1];
-            std::vector<Dim> real_lines = other_dims(g, d.size, axis, in, out), r2t, t2t, t2r;
+            std::vector<Dim> real_lines = other_dims(g, size, axis, in, out), r2t, t2t, t2r;
             uint64_t ts = nc, nlines = 1;
             for (const Dim& rl : real_lines) {
                 r2t.push_back(Dim{rl.n, rl.is, (int64_t)ts});
@@ -1624,26 +1637,29 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
                 ts *= rl.n; nlines *= rl.n;
             }
             const uint64_t region = nlines * nc;
-            g.temp_elems = std::max<uint64_t>(g.temp_elems, region);
+            g.temp_elems = std::max<uint64_t>(g.temp_elems, (uint64_t)cbase + region);
             PassReq ew;
             ew.elementwise = true; ew.store_io = io; ew.dst_flags = dflags; ew.aux0 = a0; ew.aux1 = a1;
             ew.aux_u0 = (uint32_t)N; ew.aux_u1 = (uint32_t)nc;
             ew.ew_op = 9; ew.n = (int)nc; ew.ew_items = (uint32_t)nc; ew.in_es = es_in; ew.out_es = 1;
             ew.in_role = in.role; ew.out_role = ROLE_TEMP; ew.what = "r2r (composed): operator load side";
+            ew.in_base = base; ew.out_base = cbase;
             int rc2;
             if ((rc2 = emit_ew(g, list, ew, r2t)) != R_SUCCESS) return rc2;
             list.back().in_scalar = true;
             C2CJob job;
             job.N = nc; job.inv = (type == 3) ? 1 : 0; job.es_in = job.es_out = 1; job.lines = t2t; job.unit_lines = false;
-            job.in_role = job.out_role = ROLE_TEMP; job.tmp_base = (int64_t)region; job.scale = 1.0;
+            job.in_role = job.out_role = ROLE_TEMP; job.in_base = job.out_base = cbase; job.tmp_base = cbase + (int64_t)region;
+            job.scale = 1.0;
             if ((rc2 = plan_c2c(g, list, job)) != R_SUCCESS) return rc2 == R_UNSUPPORTED_FFT_LENGTH ? R_UNSUPPORTED_FFT_LENGTH_R2R : rc2;
             const uint64_t items = (type == 3) ? nc : N;
             ew.ew_op = 10; ew.n = (int)items; ew.ew_items = (uint32_t)items; ew.in_es = 1; ew.out_es = es_out;
             ew.in_role = ROLE_TEMP; ew.out_role = out.role; ew.what = "r2r (composed): operator store side";
+            ew.in_base = cbase; ew.out_base = base;
             ew.ops = (scale != 1.0) ? B2_OP_SCALE : 0; ew.scale = scale;
             if ((rc2 = emit_ew(g, list, ew, t2r)) != R_SUCCESS) return rc2;
             list.back().out_scalar = true;
-            continue;
+            return R_SUCCESS;
         }
         if (is_dst) {   // sign / reversal wrappers (API guide :581-583)
             if (type == 2) rq.dst_flags = B2_DST_NEG_ODD_IN | B2_DST_REV_OUT;
@@ -1655,7 +1671,17 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
         rq.in_es = axis == 0 ? 1 : (int64_t)in.stride[axis - 1];
         rq.out_es = axis == 0 ? 1 : (int64_t)out.stride[axis - 1];
         rq.in_role = in.role; rq.out_role = out.role;
-        std::vector<Dim> lines = other_dims(g, d.size, axis, in, out);
+        std::vector<Dim> lines = other_dims(g, size, axis, in, out);
+        rq.in_base = rq.out_base = base;
+        if (share) {
+            // lines[0] is the x columns: share them out as pairs, then count the share's real columns again (an odd nx leaves
+            // the last pair with one column: the kernel runs it unpaired)
+            const uint64_t nx = lines[0].n, pairs = (nx + 1) / 2;
+            lines[0] = Dim{pairs, 2, 2};
+            if (share_lines(lines, d.dist_world, d.dist_rank, true, rq.in_base, rq.out_base) != R_SUCCESS) return R_UNSUPPORTED_FFT_LENGTH;
+            const bool last = lines[0].n == pairs || d.dist_rank + 1 == d.dist_world;   // the share ends with column nx-1
+            lines[0] = Dim{2 * lines[0].n - (last && nx % 2 ? 1 : 0), 1, 1};
+        }
         std::vector<Dim> m = merge_dims(lines);
         if (axis != 0) {
             if (!m.empty() && m[0].is == 1) { rq.group = m[0]; m.erase(m.begin()); }
@@ -1669,8 +1695,51 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
         rq.ops = (scale != 1.0) ? B2_OP_SCALE : 0;
         rq.scale = scale;
         rq.what = "dct axis";
-        int rc = emit(g, list, rq);
+        return emit(g, list, rq);
+    };
+
+    if (g.distributed) {
+        // Slabs along the last dimension (DESIGN section 7), in the order of the R2C slab plans: forward, the lower axes inside
+        // this rank's slab, a barrier, then the last axis over the whole window on this rank's share of its lines; the inverse
+        // runs the other way round.  The local axes keep their scratch inside the rank's temp slab: the same bytes as its data
+        // slab, in complex (temp) elements.
+        const uint32_t la = d.fft_dim - 1;
+        uint64_t lsize[B200FFT_MAX_DIMS];
+        for (int a = 0; a < B200FFT_MAX_DIMS; ++a) lsize[a] = d.size[a];
+        lsize[la] /= d.dist_world;
+        Layout slab = buf;
+        // one batch: its pitch addresses nothing, but sizes the scratch of a long strided axis -- a slab's worth, not the window
+        slab.batch_stride = lsize[la] * d.buffer_stride[la - 1];
+        const int64_t base = slab_base(g);
+        const uint64_t slab_end = ((uint64_t)base + slab.batch_stride) / 2;
+        for (size_t i = 0; i < axes.size(); ++i) {
+            const size_t before = list.size();
+            int rc;
+            if (axes[i] == la) {
+                rc = plan_axis(la, d.size, buf, buf, 0, true);
+                if (rc == R_SUCCESS && list.size() > before) list[before].sync_before = true;
+            } else {
+                const bool after_cross = inv && i > 0 && axes[i - 1] == la;
+                rc = plan_in_slab(g, list, slab_end, after_cross, [&] { return plan_axis(axes[i], lsize, slab, slab, base, false); });
+            }
+            if (rc != R_SUCCESS) return rc;
+            g.axis_uploads[inv ? 1 : 0][axes[i]] += (uint32_t)(list.size() - before);
+        }
+        return R_SUCCESS;
+    }
+    for (size_t i = 0; i < axes.size(); ++i) {
+        Layout in = buf, out = buf;
+        if (!inv) {
+            if (i == 0 && d.is_input_formatted) in = inl;
+            if (i + 1 == axes.size() && d.is_output_formatted) out = outl;
+        } else {
+            if (i == 0 && d.is_output_formatted) in = outl;
+            if (i + 1 == axes.size() && d.is_input_formatted && d.inverse_return_to_input) out = inl;
+        }
+        const size_t before = list.size();
+        const int rc = plan_axis(axes[i], d.size, in, out, 0, false);
         if (rc != R_SUCCESS) return rc;
+        g.axis_uploads[inv ? 1 : 0][axes[i]] += (uint32_t)(list.size() - before);
     }
     return R_SUCCESS;
 }
@@ -1718,16 +1787,19 @@ static int build_plan_impl(const b200fft_desc& din, PlanGraph& g) {
         if (d.dist_rank >= d.dist_world) return R_INVALID_DEVICE;
         // 1-D: one long sequence (Four-Step over the window).  2-D / 3-D: slabs along the last dimension, default strides.
         // 2-D / 3-D R2C: slabs of the in-place layout (H = nx/2+1 complex per row), pitches that may be padded; even nx > 2
-        // only, whose x axis needs no scratch beyond the rank's own slab (the odd lengths' composed path does)
-        const bool r2c_slab = d.perform_r2c && (d.fft_dim == 2 || d.fft_dim == 3);
-        if (d.fft_dim > 3 || d.number_batches * d.coordinate_features != 1 || (d.perform_r2c && !r2c_slab) || d.perform_dct ||
-            d.perform_dst || d.is_input_formatted || d.is_output_formatted || d.omit_dimension[0] ||
-            (!r2c_slab && d.buffer_stride[0] != d.size[0]))
+        // only, whose x axis needs no scratch beyond the rank's own slab (the odd lengths' composed path does).
+        // 2-D / 3-D DCT / DST: slabs of the real array (bufferStride in real elements), pitches that may be padded
+        const bool real_tf = d.perform_r2c || d.perform_dct || d.perform_dst;
+        const bool real_slab = real_tf && (d.fft_dim == 2 || d.fft_dim == 3);
+        if (d.fft_dim > 3 || d.number_batches * d.coordinate_features != 1 || (real_tf && !real_slab) ||
+            d.is_input_formatted || d.is_output_formatted || d.omit_dimension[0] ||
+            (!real_slab && d.buffer_stride[0] != d.size[0]))
             return R_UNSUPPORTED_FFT_LENGTH;
-        if (r2c_slab) {
+        if (real_slab) {
             for (uint32_t a = 0; a < d.fft_dim; ++a)
                 if (d.omit_dimension[a]) return R_UNSUPPORTED_FFT_LENGTH;
-            if (d.size[0] % 2 || d.size[0] <= 2 || d.size[d.fft_dim - 1] % d.dist_world || d.buffer_stride[0] < d.size[0] / 2 + 1 ||
+            const uint64_t row = d.perform_r2c ? d.size[0] / 2 + 1 : d.size[0];
+            if ((d.perform_r2c && (d.size[0] % 2 || d.size[0] <= 2)) || d.size[d.fft_dim - 1] % d.dist_world || d.buffer_stride[0] < row ||
                 (d.fft_dim == 3 && d.buffer_stride[1] < d.size[1] * d.buffer_stride[0]))
                 return R_UNSUPPORTED_FFT_LENGTH;
         } else if (d.fft_dim > 1) {

@@ -269,16 +269,20 @@ class FusedDistributedFFTND(FusedDistributedFFT1D):
         self.local = self.seq.tensor(torch, dt).reshape(local_shape)
 
 
-def r2c_slab_pitches(shape_xyz, world, esz, granularity):
-    """complex-element pitches (bufferStride) of the in-place R2C layout whose slabs -- n_last/world outermost indices each --
-    fill whole mapping granules: H = nx/2+1 complex per row, and only the outermost pitch of a slab (the row pitch in 2-D, the
-    plane pitch in 3-D) padded, to the smallest value that makes a slab a multiple of `granularity` bytes.  Whenever n_last/world
-    is a power of two that adds less than one granule per slab."""
+def r2c_slab_pitches(shape_xyz, world, esz, granularity, real=False):
+    """pitches (bufferStride) of a real transform's slab layout whose slabs -- n_last/world outermost indices each -- fill whole
+    mapping granules.  R2C (default): complex elements of the in-place layout, H = nx/2+1 per row.  `real=True` (DCT / DST): real
+    elements, nx per row.  Only the outermost pitch of a slab (the row pitch in 2-D, the plane pitch in 3-D) is padded, to the
+    smallest value that makes a slab a multiple of `granularity` bytes and keeps the pitch even in real elements (the complex view
+    of neighbouring column pairs needs even pitches).  Whenever n_last/world is a power of two that adds less than one granule per
+    slab."""
     import math
     nx, rows = shape_xyz[0], shape_xyz[-1] // world
-    h = nx // 2 + 1
+    h = nx if real else nx // 2 + 1
     inner = h if len(shape_xyz) == 2 else h * shape_xyz[1]
     step = granularity // math.gcd(granularity, rows * esz)       # pitch multiple that makes rows * pitch * esz whole granules
+    if real and step % 2:
+        step *= 2
     outer = -(-inner // step) * step
     return [outer, outer * shape_xyz[1]] if len(shape_xyz) == 2 else [h, outer, outer * shape_xyz[2]]
 
@@ -334,3 +338,49 @@ class FusedDistributedRFFTND(FusedDistributedFFT1D):
         self.real = self.seq.tensor(torch, rdt).as_strided((rows,) + inner + (shape_xyz[0],),
                                                            tuple(2 * p for p in (self.pitches[nd - 2],) + inner_pitch) + (1,))
 
+
+
+class FusedDistributedR2RND(FusedDistributedFFT1D):
+    """A 2-D or 3-D DCT or DST (types 1-4) whose real array is spread over the GPUs of a box in slabs along its last dimension,
+    like FusedDistributedRFFTND.
+
+    `shape_xyz` = (nx, ny[, nz]) with x fastest; `kind` the transform type, `dst` a DST instead of a DCT.  Rank g holds the
+    last-dimension indices [g*n/R, (g+1)*n/R) in `self.local`, shape (n/R, [ny,] nx): a strided view whose outermost pitch is padded
+    (`pitches`, real elements: r2c_slab_pitches) so that the slab maps onto whole granules of the peer window.
+
+    `self()` runs the forward transform, `self(inverse=True)` the inverse type (DCT-II <-> DCT-III, types 1 and 4 their own inverse;
+    scaled per axis by 1/(2N), 1/(2(N-1)) for DCT-I or 1/(2(N+1)) for DST-I with `normalize`), in place and asynchronously on the
+    current stream.  Forward: the lower axes inside the slab, a device-side barrier, the last axis across the slabs on this rank's
+    share of the columns; the inverse the other way round."""
+
+    def __init__(self, shape_xyz, dist, device, kind=2, dst=False, double=False, normalize=False):
+        import torch
+        from . import api, _lib
+        self.torch, self.dist, self.api = torch, dist, api
+        self.R, self.r = dist.get_world_size(), dist.get_rank()
+        shape_xyz = tuple(int(v) for v in shape_xyz)
+        if not 2 <= len(shape_xyz) <= 3:
+            raise ValueError("2-D or 3-D shapes")
+        if kind not in (1, 2, 3, 4):
+            raise ValueError("kind must be 1, 2, 3 or 4")
+        if shape_xyz[-1] % self.R:
+            raise ValueError("world size must divide the last dimension")
+        esz = 8 if double else 4
+        gran = int(_lib.load().b200fft_window_granularity(int(device)))
+        if gran == 0:
+            raise RuntimeError("CUDA virtual memory management is not available on this device")
+        self.shape_xyz = shape_xyz
+        self.pitches = r2c_slab_pitches(shape_xyz, self.R, esz, gran, real=True)
+        rows = shape_xyz[-1] // self.R
+        nd = len(shape_xyz)
+        self.n = 1
+        for v in shape_xyz:
+            self.n *= v
+        cfg = api.VkFFTConfiguration(FFTdim=nd, size=list(shape_xyz), performDCT=0 if dst else kind, performDST=kind if dst else 0,
+                                     bufferStride=list(self.pitches), device=device, doublePrecision=int(double),
+                                     normalize=int(normalize), userTempBuffer=1, distWorld=self.R, distRank=self.r)
+        self._open(rows * self.pitches[nd - 2] * esz, cfg, device)
+        inner = tuple(reversed(shape_xyz[1:-1]))                          # (ny,) in 3-D
+        inner_pitch = tuple(self.pitches[:nd - 2][::-1])                  # (nx,) in 3-D
+        self.local = self.seq.tensor(torch, torch.float64 if double else torch.float32).as_strided(
+            (rows,) + inner + (shape_xyz[0],), (self.pitches[nd - 2],) + inner_pitch + (1,))
