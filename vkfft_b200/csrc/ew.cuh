@@ -23,7 +23,8 @@ enum { B2_EW_COPY_MUL = 0, B2_EW_R2C_POST = 1, B2_EW_C2R_PRE = 2,
        // their own around a C2C plan on scratch (one real line per complex line).  store_io = B2_IO_DCT1/2/3/DCT4_ODD/DST1,
        // aux_u0 = logical real length N, aux_u1 = complex length, dst_flags as in generic.cuh
        B2_EW_R2R_PRE = 9, B2_EW_R2R_POST = 10,
-       B2_EW_ZERO = 11 };          // clear P.n items of every line (aux_u0 = 1: items and strides count scalars, not complex elements)
+       B2_EW_ZERO = 11,            // clear P.n items of every line (aux_u0 = 1: items and strides count scalars, not complex elements)
+       B2_EW_CONV_REAL = 12 };     // B2_EW_CONV on real elements (DCT / DST spectra): offsets and strides count scalars
 // B2_EW_CONV packs its options into aux_u0: bits 0-7 features per vector, 8-11 matrix size (0 = per-feature product),
 // 12 symmetric kernel, 13-14 conjugation (1 sequence, 2 kernel), 15 cross-power-spectrum normalisation; aux_u1 = kernels
 enum { B2_CONV_SYM = 1u << 12, B2_CONV_CONJ_SEQ = 1u << 13, B2_CONV_CONJ_KER = 1u << 14, B2_CONV_XPS = 1u << 15 };
@@ -72,6 +73,47 @@ struct Elementwise {
                 const X zc = f(xc, conj(xk), ld_lut(w + kc));
                 stx(out + (int64_t)k * P.out_es, zk);
                 if (kc != k && kc != n) stx(out + (int64_t)kc * P.out_es, zc);
+            }
+        }
+    }
+
+    // B2_EW_CONV on real elements (DCT / DST spectra): the same layout rules, offsets and strides in scalars, and no
+    // conjugation or normalisation options.  The vector is held in named registers rather than an array, so that this
+    // operation adds no stack frame to the kernel the other operations share.
+    B2_D static void conv_real(const b2_pass_params& P, int64_t in_off, int64_t out_off, uint32_t j0) {
+        const T* rin = (const T*)P.in + in_off;
+        T* rout = (T*)P.out + out_off;
+        const uint32_t C = P.aux_u0 & 0xff, M = (P.aux_u0 >> 8) & 0xf, NK = P.aux_u1 ? P.aux_u1 : 1;
+        const bool sym = (P.aux_u0 & B2_CONV_SYM) != 0;
+        const int64_t batch_stride = (int64_t)C * P.in_es;
+        const T* __restrict__ ker = (const T*)P.aux0 + in_off % batch_stride;
+        const uint32_t kplanes = M >= 2 ? (sym ? M * (M + 1) / 2 : M * M) : C;
+#pragma unroll 2
+        for (int i = 0; i < B2_EW_PER_THREAD; ++i) {
+            const uint32_t j = j0 + i * B2_EW_THREADS;
+            if (j >= P.n) break;
+            if (M >= 2) {
+                const T x0 = rin[j], x1 = rin[P.in_es + j], x2 = M > 2 ? rin[2 * P.in_es + j] : T(0);
+                for (uint32_t k = 0; k < NK; ++k) {
+                    const T* kk = ker + (int64_t)k * kplanes * P.out_es + j;
+                    auto w = [&](uint32_t r, uint32_t c) {
+                        uint32_t idx;
+                        if (sym) { const uint32_t a = r < c ? r : c, b = r < c ? c : r; idx = a * M - a * (a - 1) / 2 + (b - a); }
+                        else idx = r * M + c;
+                        return kk[(int64_t)idx * P.out_es];
+                    };
+                    for (uint32_t r = 0; r < M; ++r) {
+                        T acc = w(r, 0) * x0 + w(r, 1) * x1;
+                        if (M > 2) acc += w(r, 2) * x2;
+                        rout[(int64_t)k * batch_stride + (int64_t)r * P.in_es + j] = acc;
+                    }
+                }
+            } else {
+                for (uint32_t c = 0; c < C; ++c) {
+                    const T xv = rin[(int64_t)c * P.in_es + j];
+                    for (uint32_t k = 0; k < NK; ++k)
+                        rout[(int64_t)k * batch_stride + (int64_t)c * P.in_es + j] = ker[(int64_t)(k * kplanes + c) * P.out_es + j] * xv;
+                }
             }
         }
     }
@@ -247,6 +289,8 @@ struct Elementwise {
                     }
                 }
             }
+        } else if (P.load_io == B2_EW_CONV_REAL) {
+            conv_real(P, in_off, out_off, j0);
         } else if (P.load_io == B2_EW_DCT2_POST_COLS || P.load_io == B2_EW_DCT3_PRE_COLS) {
             // this CTA's "line" is row k = gl of a complex-view column block; its partner is row N-k (N = aux_u0);
             // items are the columns (unit stride).  aux0[k] = e^{-i pi k/2N}

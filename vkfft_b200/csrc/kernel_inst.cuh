@@ -151,7 +151,7 @@ struct Registrar {
     using KT = KindTraits<KIND>;
     using Sch = RList<Rs...>;
     static constexpr int RMODE = (OPS & B2_OP_REAL_EVEN) ? (INV ? 2 : 1)
-                               : ((OPS & B2_OP_DCT23) ? (INV ? 4 : 3) : ((OPS & B2_OP_PERM_IN) ? 5 : ((OPS & B2_OP_PERM_OUT) ? 6 : ((OPS & B2_OP_BLUESTEIN) ? (INV ? 8 : 7) : ((OPS & B2_OP_CONV) ? 9 : ((OPS & B2_OP_BLUE_FUSED) ? 11 : 0))))));
+                               : ((OPS & B2_OP_DCT23) ? ((OPS & B2_OP_CONV) ? 12 : (INV ? 4 : 3)) : ((OPS & B2_OP_PERM_IN) ? 5 : ((OPS & B2_OP_PERM_OUT) ? 6 : ((OPS & B2_OP_BLUESTEIN) ? (INV ? 8 : 7) : ((OPS & B2_OP_CONV) ? 9 : ((OPS & B2_OP_BLUE_FUSED) ? 11 : 0))))));
     static constexpr int ST = ((OPS & B2_OP_HALF_IN) ? 1 : 0) | ((OPS & B2_OP_HALF_OUT) ? 2 : 0);   // half-precision storage
     using C = KCfg<T, Sch, TPL, Q, V, KT::LMAP, KT::SMAP, KT::LAYOUT, INV, (OPS & B2_OP_TWIDDLE_OUT), KT::IN_UNIT, KT::OUT_UNIT,
                    MINB, RMODE, ST>;
@@ -288,7 +288,8 @@ template <int KIND, typename T, int TPL, int Q, int V, int MINB, int... Rs>
 struct MaybeDct<true, KIND, T, TPL, Q, V, MINB, Rs...> {
     Registrar<KIND, T, TPL, Q, V, MINB, false, B2_OP_DCT23, Rs...> d2;
     Registrar<KIND, T, TPL, Q, V, MINB, true, B2_OP_DCT23, Rs...> d3;
-    explicit MaybeDct(const char* n) : d2(n), d3(n) {}
+    Registrar<KIND, T, TPL, Q, V, MINB, false, B2_OP_DCT23 | B2_OP_CONV, Rs...> cv;   // DCT / DST convolution (RMODE 12)
+    explicit MaybeDct(const char* n) : d2(n), d3(n), cv(n) {}
 };
 }  // namespace b200fft
 // factor kernels of the long strided DCT-II/III Four-Step: (forward, phase + permuted gather) and (inverse, permuted scatter)

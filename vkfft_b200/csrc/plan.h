@@ -106,6 +106,7 @@ struct PlanGraph {
     uint64_t algorithmic_bytes = 0;
     uint32_t axis_uploads[2][B200FFT_MAX_DIMS] = {{0, 0, 0, 0}, {0, 0, 0, 0}};   // launches per axis, [0] forward / [1] inverse (the reference's numAxisUploads)
     int skip_axis = -1;          // convolution plans: this axis is transformed by the fused kernel, the direction planners leave it out
+    int conv_axis = -1;          // DCT / DST convolution: plan_direction_dct plans only this axis, as the fused convolution launch
     uint64_t ctl_words = 0;      // control block of the fused Four-Step launches (largest one of the plan)
     // half-precision storage (desc.precision = B200FFT_F16: the reference's halfPrecision, vkFFT_Structs.h:210): arithmetic, tables
     // and g.prec are FP32, the elements of the flagged buffer roles are 32-bit (half re, half im); strides / offsets count elements

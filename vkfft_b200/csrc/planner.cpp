@@ -1436,9 +1436,10 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
     const bool is_dst = d.perform_dst != 0;
     int type = (int)(is_dst ? d.perform_dst : d.perform_dct);
     if (inv && (type == 2 || type == 3)) type = 5 - type;
+    const bool conv = g.conv_axis >= 0;   // type-2 forward, kernel product and type-3 inverse of this axis in one launch
     std::vector<uint32_t> axes;
     for (uint32_t a = 0; a < d.fft_dim; ++a)
-        if (!d.omit_dimension[a] && d.size[a] > 1) axes.push_back(a);
+        if (!d.omit_dimension[a] && d.size[a] > 1 && (int)a != g.skip_axis && (!conv || (int)a == g.conv_axis)) axes.push_back(a);
     if (inv) std::reverse(axes.begin(), axes.end());
     // out of place: the same data flow as plan_direction_c2c -- the first axis reads the formatted source, the last axis
     // writes the formatted destination, everything in between lives in `buffer`.  No launch writes the source.
@@ -1453,7 +1454,7 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
         const uint64_t N = size[axis];
         const int64_t cbase = (base + 1) / 2;   // first element of the slab in complex units (scratch, complex view)
         double scale = 1.0;
-        if (inv && d.normalize) scale = 1.0 / (type == 1 ? (is_dst ? 2.0 * (double)(N + 1) : 2.0 * (double)(N - 1)) : 2.0 * (double)N);
+        if ((inv || conv) && d.normalize) scale = 1.0 / (type == 1 ? (is_dst ? 2.0 * (double)(N + 1) : 2.0 * (double)(N - 1)) : 2.0 * (double)N);
         uint64_t n;
         PassReq rq;
         rq.force_generic = true;
@@ -1476,16 +1477,23 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
         }
         // DCT-II/III on the specialised kernels: contiguous real lines (axis 0) or pairs of neighbouring real columns
         // viewed as one complex column (other axes)
-        if (!is_dst && (type == 2 || type == 3)) {
+        if (conv || (!is_dst && (type == 2 || type == 3))) {
             const int kkind = axis == 0 ? B2_KIND_ROWS : B2_KIND_COLS;
             const int kinv = type == 3 ? 1 : 0;
             std::vector<Dim> lines = other_dims(g, size, axis, in, out);
-            bool ok = b2_find_kernel(kkind, g.prec, (int)N, kinv, B2_OP_DCT23) != nullptr;
+            const int cop = conv ? B2_OP_CONV : 0;
+            bool ok = b2_find_kernel(kkind, g.prec, (int)N, kinv, B2_OP_DCT23 | cop) != nullptr;
             PassReq fr;
-            fr.kind = kkind; fr.n = (int)N; fr.inv = kinv; fr.ops = B2_OP_DCT23 | ((scale != 1.0) ? B2_OP_SCALE : 0);
+            fr.kind = kkind; fr.n = (int)N; fr.inv = kinv; fr.ops = B2_OP_DCT23 | cop | ((scale != 1.0) ? B2_OP_SCALE : 0);
             fr.scale = scale; fr.aux0 = aux_for(g, AUX_DCT23, N);
             fr.in_role = in.role; fr.out_role = out.role;
             fr.what = "dct axis (fused)";
+            if (conv) {
+                // the kernel operand takes aux0 (ROLE_KERNEL), the phase table aux1; DST-II -> DST-III through the flags
+                fr.aux1 = fr.aux0; fr.aux0 = -1;
+                fr.dst_flags = is_dst ? (B2_DST_NEG_ODD_IN | B2_DST_REV_OUT | B2_DST_ALT_OUT) : 0;
+                fr.what = "fused r2r convolution (dct-ii, kernel product, dct-iii)";
+            }
             // complex view of the real data (pairs of neighbouring columns): size[0] and every stride of both sides even
             auto even_view = [&](const Layout& l) {
                 bool e = l.batch_stride % 2 == 0;
@@ -1528,7 +1536,7 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
             // permutation folded into the first gather (DCT-II) / the last scatter (DCT-III) and a separate split/merge launch
             bool long_strided = false;
             uint64_t L1 = 0, L2 = 0;
-            if (view_ok && N % 2 == 0) {
+            if (!conv && view_ok && N % 2 == 0) {
                 const b2_kernel_info* single = b2_find_kernel(B2_KIND_COLS, g.prec, (int)N, kinv, B2_OP_DCT23);
                 if (!single || single->q < 8) {
                     uint64_t bestc = ~0ull;
@@ -1609,6 +1617,7 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
                 return R_SUCCESS;
             }
             if (ok) return emit(g, list, fr);
+            if (conv) return R_UNSUPPORTED_FFT_LENGTH;
         }
         if (n < 2) return R_UNSUPPORTED_FFT_LENGTH_R2R;
         if (!is_smooth(n) || !generic_fits(g, n)) {
@@ -1730,7 +1739,7 @@ int plan_direction_dct(PlanGraph& g, std::vector<PassPlan>& list, int inv) {
     for (size_t i = 0; i < axes.size(); ++i) {
         Layout in = buf, out = buf;
         if (!inv) {
-            if (i == 0 && d.is_input_formatted) in = inl;
+            if (i == 0 && d.is_input_formatted && !conv) in = inl;   // the fused launch reads what the other axes wrote to `buffer`
             if (i + 1 == axes.size() && d.is_output_formatted) out = outl;
         } else {
             if (i == 0 && d.is_output_formatted) in = outl;
@@ -1902,14 +1911,19 @@ static int build_plan_impl(const b200fft_desc& din, PlanGraph& g) {
         // vkFFT_Convolution.h:125 -- here it is its own streaming launch)
         const uint64_t C = d.coordinate_features, B = d.number_batches, NK = d.number_kernels ? d.number_kernels : 1;
         const uint32_t M = d.matrix_convolution >= 2 ? d.matrix_convolution : 0;
-        if (d.perform_dct || d.perform_dst || d.is_output_formatted || d.dist_world > 1) return R_UNSUPPORTED_FFT_LENGTH;
-        for (uint32_t a = 0; a < d.fft_dim; ++a) if (d.omit_dimension[a]) return R_UNSUPPORTED_FFT_OMIT;
+        // DCT / DST: forward type-k transform, product with a real kernel in the buffer's layout, inverse transform (the
+        // inverse pairs and normalisation of plan_direction_dct).  Conjugation and cross-power normalisation have no meaning
+        // for real spectra.
+        const bool r2r = d.perform_dct || d.perform_dst;
+        if (d.is_output_formatted || d.dist_world > 1) return R_UNSUPPORTED_FFT_LENGTH;
+        if (r2r && (d.conjugate_convolution || d.cross_power_spectrum_normalization)) return R_UNSUPPORTED_FFT_LENGTH;
+        for (uint32_t a = 0; a < d.fft_dim; ++a) if (d.omit_dimension[a]) return r2r ? R_UNSUPPORTED_FFT_LENGTH : R_UNSUPPORTED_FFT_OMIT;
         if (M > 3 || (M && C != M) || C > 255 || (NK > 1 && B > 1)) return R_UNSUPPORTED_FFT_LENGTH;
         g.has_fwd = true; g.has_inv = false;
         // Fused last axis: per-feature product, one kernel set, packed layout, and a fused kernel for the length of the
         // last transformed axis (contiguous lines in 1-D, strided axis otherwise).  That launch runs the axis forward,
         // multiplies and runs it inverse; the remaining axes keep their ordinary forward / inverse passes around it.
-        {
+        if (!r2r) {
             const uint32_t la = d.fft_dim - 1;
             bool packed = !d.is_output_formatted && (la > 0 || (!d.perform_r2c && !d.is_input_formatted));
             uint64_t want = d.perform_r2c ? d.size[0] / 2 + 1 : d.size[0];
@@ -1953,11 +1967,51 @@ static int build_plan_impl(const b200fft_desc& din, PlanGraph& g) {
                 return R_SUCCESS;
             }
         }
+        if (r2r) {
+            // Fused last axis of a DCT-II / DST-II convolution under the C2C conditions (packed layout, one kernel set, no
+            // matrix, a kernel for the length): DCT-II forward, pair pass with the kernel product, DCT-III inverse in one
+            // launch (stockham.cuh RMODE 12), the other axes keep their R2R passes around it: 2*nd-1 launches.
+            const uint32_t la = d.fft_dim - 1;
+            const int kind = (int)(d.perform_dst ? d.perform_dst : d.perform_dct);
+            bool packed = la > 0 || !d.is_input_formatted;
+            uint64_t want = d.size[0];
+            for (uint32_t a = 0; a < d.fft_dim && packed; ++a) { packed = d.buffer_stride[a] == want; want *= (a + 1 < d.fft_dim ? d.size[a + 1] : 1); }
+            const uint64_t KS = C * d.buffer_stride[la];
+            const int ckind = la == 0 ? B2_KIND_ROWS : B2_KIND_COLS;
+            if (kind == 2 && packed && !M && NK == 1 && d.size[la] > 1 && d.size[la] <= 0x7fffffff && KS < (1ull << 32) &&
+                (la == 0 || d.size[0] % 2 == 0) && !getenv("B200FFT_NO_FUSED_CONV") &&
+                b2_find_kernel(ckind, g.prec, (int)d.size[la], 0, B2_OP_DCT23 | B2_OP_CONV)) {
+                g.batches = B * C;
+                g.skip_axis = (int)la;
+                rc = plan(g.fwd, 0);
+                g.skip_axis = -1;
+                if (rc != R_SUCCESS) return rc;
+                const size_t before = g.fwd.size();
+                g.conv_axis = (int)la;
+                rc = plan_direction_dct(g, g.fwd, 0);
+                g.conv_axis = -1;
+                if (rc != R_SUCCESS) return rc;
+                for (size_t i = before; i < g.fwd.size(); ++i) {
+                    g.fwd[i].aux0_role = ROLE_KERNEL;
+                    g.fwd[i].P.in_len = (uint32_t)KS;          // the kernel's features x plane block, in real elements
+                }
+                std::vector<PassPlan> tail;
+                b200fft_desc back = g.desc;
+                g.desc.is_input_formatted = 0; g.desc.inverse_return_to_input = 0;
+                g.skip_axis = (int)la;
+                rc = plan(tail, 1);
+                g.skip_axis = -1;
+                g.desc = back;
+                if (rc != R_SUCCESS) return rc;
+                g.fwd.insert(g.fwd.end(), tail.begin(), tail.end());
+                return R_SUCCESS;
+            }
+        }
         g.batches = B * C;
         if ((rc = plan(g.fwd, 0)) != R_SUCCESS) return rc;
         const uint64_t plane = d.buffer_stride[d.fft_dim - 1];
         PassReq cv;
-        cv.elementwise = true; cv.ew_op = 5 /* B2_EW_CONV */;
+        cv.elementwise = true; cv.ew_op = r2r ? 12 /* B2_EW_CONV_REAL */ : 5 /* B2_EW_CONV */;
         cv.n = (int)std::min<uint64_t>(plane, 0x7fffffff); cv.ew_items = (uint32_t)plane;
         if (plane > 0x7fffffffull) return R_UNSUPPORTED_FFT_LENGTH;
         cv.in_es = cv.out_es = (int64_t)plane;
@@ -1965,7 +2019,7 @@ static int build_plan_impl(const b200fft_desc& din, PlanGraph& g) {
                     (d.conjugate_convolution == 2 ? (1u << 14) : 0) | (d.cross_power_spectrum_normalization ? (1u << 15) : 0);
         cv.aux_u1 = (uint32_t)NK;
         cv.in_role = cv.out_role = ROLE_BUFFER;
-        cv.what = "convolution: spectrum x kernel";
+        cv.what = r2r ? "convolution: real spectrum x kernel" : "convolution: spectrum x kernel";
         std::vector<Dim> cvl;
         {
             // packed layout: one line = one plane.  Padded pitches: one line = one row, so that the gaps between rows and planes
@@ -1981,6 +2035,7 @@ static int build_plan_impl(const b200fft_desc& din, PlanGraph& g) {
         cvl.push_back(Dim{B, (int64_t)(C * plane), (int64_t)(C * plane)});      // kernel k writes output batch k (one input, NK outputs)
         if ((rc = emit_ew(g, g.fwd, cv, cvl)) != R_SUCCESS) return rc;
         g.fwd.back().aux0_role = ROLE_KERNEL;
+        g.fwd.back().in_scalar = g.fwd.back().out_scalar = r2r;
         // the inverse runs in `buffer` on every output batch
         b200fft_desc back = g.desc;
         g.desc.is_input_formatted = 0; g.desc.inverse_return_to_input = 0;

@@ -130,10 +130,11 @@ struct KCfg {
     static constexpr int QP = Q;  // elem-major row pitch
     // 3: DCT-II, 4: DCT-III with two real lines per complex line (contiguous real lines, or neighbouring real columns
     //    viewed as one complex column on strided axes) -- vkFFT_R2R.h:193-229, :784-859 as fused load/store stages
+    // 12: DCT / DST convolution: DCT-II forward, kernel product in the tile, DCT-III inverse (layouts of 3 / 4)
     // 10: short contiguous lines, one thread per line, staged through shared memory so that HBM is read and written in
     //     whole consecutive segments (thread q alone would walk its line in 8-byte steps N*8 bytes apart from its neighbour)
     static constexpr int SMEM_ELEMS = RMODE == 10 ? Q * (N + 1)
-                                    : ((Sch::ns <= 1 && RMODE != 1 && RMODE != 3 && RMODE != 4) ? 0 : ((LAYOUT == LAY_LINE) ? Q * LS : N * QP));
+                                    : ((Sch::ns <= 1 && RMODE != 1 && RMODE != 3 && RMODE != 4 && RMODE != 12) ? 0 : ((LAYOUT == LAY_LINE) ? Q * LS : N * QP));
     static constexpr int SMEM_BYTES = SMEM_ELEMS * 2 * (int)sizeof(T);
     // stage twiddles w^k generated from w^1, w^2, w^4, w^8 (Engine::compute): 4 table loads instead of 15 per radix-16
     // butterfly; every kernel generates them.
@@ -460,10 +461,11 @@ struct Engine {
                     const int p = b + k * NB;
                     X z = mk<T>(T(0), T(0));
                     if (ok) {
-                        if constexpr (C::RMODE == 3) {
+                        if constexpr (C::RMODE == 3 || C::RMODE == 12) {
                             const int src = makhoul(p);
                             if constexpr (C::LAYOUT == LAY_LINE) { z.x = la[src]; if (vb) z.y = lb[src]; }
                             else z = lc[(int64_t)src * P.in_es];
+                            if (C::RMODE == 12 && (P.dst_flags & B2_DST_NEG_ODD_IN) && (src & 1)) z = mk<T>(-z.x, -z.y);
                         } else {
                             T a0, a1 = T(0), b0, b1 = T(0);
                             if constexpr (C::LAYOUT == LAY_LINE) {
@@ -499,7 +501,8 @@ struct Engine {
         } else {
             oc = (X*)P.out + obase_out + (int64_t)gl * P.out_gs;
         }
-        if constexpr (C::RMODE == 4 && C::LAYOUT == LAY_LINE && B2_DCT3_STAGE_OUT) {
+        const T alt = (C::RMODE == 12 && (P.dst_flags & B2_DST_ALT_OUT)) ? T(-1) : T(1);   // DST-III: odd outputs negated
+        if constexpr ((C::RMODE == 4 || C::RMODE == 12) && C::LAYOUT == LAY_LINE && B2_DCT3_STAGE_OUT) {
             // Makhoul scatter through the tile: natural-order spectrum in, coalesced 4-byte stores out
 #pragma unroll
             for (int m = 0; m < BPT; ++m) {
@@ -519,11 +522,12 @@ struct Engine {
             if (!valid) return;
 #pragma unroll 8
             for (int j = t; j < N; j += TPL) {
-                const X u = B2_SMEM_LD(sm, sidx(q, unmakhoul(j)));
+                X u = B2_SMEM_LD(sm, sidx(q, unmakhoul(j)));
+                if (j & 1) u = u * alt;
                 oa[j] = u.x;
                 if (vb) ob[j] = u.y;
             }
-        } else if constexpr (C::RMODE == 4) {
+        } else if constexpr (C::RMODE == 4 || C::RMODE == 12) {
 #pragma unroll
             for (int m = 0; m < BPT; ++m) {
 #pragma unroll
@@ -535,6 +539,7 @@ struct Engine {
                         X u = swp(x[(m * V + v) * r + k]);
                         if (do_scale) u = u * sc;
                         const int dst = makhoul(b + k * NB);
+                        if (dst & 1) u = u * alt;
                         if constexpr (C::LAYOUT == LAY_LINE) { oa[dst] = u.x; if (vb) ob[dst] = u.y; }
                         else oc[(int64_t)dst * P.out_es] = u;
                     }
@@ -563,6 +568,68 @@ struct Engine {
                 if (do_scale) { ya *= sc; yb *= sc; }
                 if constexpr (C::LAYOUT == LAY_LINE) { oa[k] = ya; if (vb) ob[k] = yb; }
                 else oc[(int64_t)k * P.out_es] = mk<T>(ya, yb);
+            }
+        }
+    }
+
+    // ---- last-stage registers -> the tile in natural order (element p at sidx(q, p)) ----------------------------------
+    template <int s>
+    B2_D static void store_smem_nat(const X* x, X* sm, int q, int t) {
+        constexpr int r = Sch::r(s), NB = nbut<s>(), BPT = bpt<s>();
+#pragma unroll
+        for (int m = 0; m < BPT; ++m) {
+#pragma unroll
+            for (int v = 0; v < V; ++v) {
+                const int b = V * (t + m * TPL) + v;
+                if (guarded<s>() && b >= NB) continue;
+#pragma unroll
+                for (int k = 0; k < r; ++k) B2_SMEM_ST(sm, sidx(q, b + k * NB), x[(m * V + v) * r + k]);
+            }
+        }
+    }
+
+    // ---- DCT / DST convolution (RMODE 12): pair pass between the DCT-II forward and the DCT-III inverse -----------------
+    // The tile holds V = FFT of the Makhoul-gathered pair of real lines (a + i b).  Each thread takes index pairs (k, N-k)
+    // of its line: the DCT-II coefficients of both real lines (the store of B2_IO_DCT2), times the two kernel lines, then
+    // the DCT-III pre-phase and merge (the load of B2_IO_DCT3), swapped for the inverse stages, written back in place.
+    // Kernel: real elements at the data's own offsets (the store side) modulo P.in_len = features x plane elements;
+    // DST (B2_DST_REV_OUT): the DST spectrum index of DCT position k is N-1-k.
+    B2_D static void pair_pass(X* sm, const b2_pass_params& P, int64_t obase_out, uint32_t gl, int q, int t, bool valid) {
+        const X* __restrict__ c = (const X*)P.aux1;
+        const uint64_t ks = P.in_len ? P.in_len : 1;
+        const bool rev = (P.dst_flags & B2_DST_REV_OUT) != 0;
+        const T* ka = nullptr; const T* kb = nullptr; const X* kc = nullptr;
+        bool vb = false;
+        if constexpr (C::LAYOUT == LAY_LINE) {
+            const int64_t oa = obase_out + (int64_t)gl * P.out_gs;
+            ka = (const T*)P.aux0 + (int64_t)((uint64_t)oa % ks);
+            kb = (const T*)P.aux0 + (int64_t)((uint64_t)(oa + P.aux_u2) % ks);
+            vb = valid && (2 * gl + 1 < P.aux_u0);
+        } else {
+            kc = (const X*)P.aux0 + (int64_t)((uint64_t)(obase_out + (int64_t)gl * P.out_gs) % (ks / 2));
+            vb = valid;
+        }
+        auto kern = [&](int j, T& wa, T& wb) {
+            const int jj = rev ? N - 1 - j : j;
+            wa = T(0); wb = T(0);
+            if (!valid) return;
+            if constexpr (C::LAYOUT == LAY_LINE) { wa = ka[jj]; if (vb) wb = kb[jj]; }
+            else { const X w = ld_lut(kc + (int64_t)jj * P.out_es); wa = w.x; wb = w.y; }
+        };
+        for (int k = t; 2 * k <= N; k += TPL) {
+            const int kp = k == 0 ? 0 : N - k;
+            const X a = B2_SMEM_LD(sm, sidx(q, k)), b = B2_SMEM_LD(sm, sidx(q, kp));
+            const X ck = ld_lut(c + k), cp = ld_lut(c + kp);
+            T wa, wb, pa, pb;
+            kern(k, wa, wb);
+            kern(kp, pa, pb);
+            const T ya = (ck * (a + conj(b))).x * wa, yb = (ck * (a - conj(b))).y * wb;          // DCT-II of line a / b at k
+            const T za = (cp * (b + conj(a))).x * pa, zb = (cp * (b - conj(a))).y * pb;          // ... at N-k
+            if (k == 0) {
+                B2_SMEM_ST(sm, sidx(q, 0), swp(mulc(mk<T>(ya, yb), ck)));
+            } else {
+                B2_SMEM_ST(sm, sidx(q, k), swp(mulc(mk<T>(ya + zb, yb - za), ck)));
+                if (kp != k) B2_SMEM_ST(sm, sidx(q, kp), swp(mulc(mk<T>(za + yb, zb - ya), cp)));
             }
         }
     }
@@ -985,6 +1052,55 @@ struct Engine {
                         }
                     }
                 }
+            }
+        } else if constexpr (C::RMODE == 12) {
+            // ---- DCT / DST convolution of the last axis in one launch: DCT-II forward stages, pair pass through the tile,
+            //      DCT-III inverse stages (forward stages on swapped values) and the DCT-III scatter with this axis's scale
+            constexpr int s = NS - 1;
+            int qs, ts;
+            tmap<C::SMAP>(tid, qs, ts);
+            const uint32_t gs = grp * Q + qs;
+            {
+                X x[bpt<0>() * V * Sch::r(0)];
+                load_global_dct<0>(x, P, obase_in, gl, tl, gl < P.G);
+                compute<0>(x, lut, tl);
+                if constexpr (NS == 1) {
+                    store_smem_nat<0>(x, sm, ql, tl);
+                } else {
+                    store_smem<0>(x, sm, ql, tl);
+                }
+            }
+            __syncthreads();
+            if constexpr (NS > 1) {
+                middle<1>(sm, lut, tid);
+                X x[bpt<s>() * V * Sch::r(s)];
+                load_smem<s>(x, sm, qs, ts);
+                compute<s>(x, lut, ts);
+                __syncthreads();
+                store_smem_nat<s>(x, sm, qs, ts);
+                __syncthreads();
+            }
+            pair_pass(sm, P, obase_out, gl, ql, tl, gl < P.G);
+            __syncthreads();
+            {
+                X x[bpt<0>() * V * Sch::r(0)];
+                load_smem<0>(x, sm, ql, tl);
+                compute<0>(x, lut, tl);
+                __syncthreads();
+                if constexpr (NS == 1) {
+                    store_global_dct<0>(x, sm, P, obase_out, gl, ql, tl, gl < P.G);
+                } else {
+                    store_smem<0>(x, sm, ql, tl);
+                }
+            }
+            if constexpr (NS > 1) {
+                __syncthreads();
+                middle<1>(sm, lut, tid);
+                X x[bpt<s>() * V * Sch::r(s)];
+                load_smem<s>(x, sm, qs, ts);
+                compute<s>(x, lut, ts);
+                __syncthreads();
+                store_global_dct<s>(x, sm, P, obase_out, gs, qs, ts, gs < P.G);
             }
         } else if constexpr (C::RMODE == 4 && C::LAYOUT == LAY_LINE && B2_DCT3_STAGE_IN) {
             // real lines staged through the tile (see stage_in_dct); every stage reads its legs from shared memory

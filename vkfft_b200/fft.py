@@ -10,6 +10,7 @@ This module gives the same surface over the C ABI:
     h = vkfft.rfftn(r, ndim=2)        # real -> half-Hermitian complex (last axis n//2+1)
     r2 = vkfft.irfftn(h, ndim=2, n_last=r.shape[-1])
     c = vkfft.dctn(r, dct_type=2)     # FFTW REDFT10 convention, idctn / dstn / idstn likewise (out of place: r is not written)
+    u = vkfft.convolve_r2r(r, k, ndim=2)   # idctn(dctn(r) * k) in one convolution plan (dst=True: DST)
 
 `ndim` = number of trailing dimensions to transform (the fast axes; leading dimensions are batches), as in pyvkfft.
 `norm`: 0 = nothing (the library's own convention: unnormalised inverse), 1 = backward transform scaled by 1/N (numpy's
@@ -278,3 +279,45 @@ def dstn(src, dest=None, ndim=None, norm=1, dst_type=2, cuda_stream=None):
 
 def idstn(src, dest=None, ndim=None, norm=1, dst_type=2, cuda_stream=None):
     return _r2r(src, dest, ndim, norm, cuda_stream, True, dst_type, True)
+
+
+def convolve_r2r(src, kernel, dest=None, ndim=None, kind=2, dst=False, norm=1, cuda_stream=None):
+    """forward DCT (DST with dst=True) of type `kind` over the last `ndim` dimensions, product with the real multiplier
+    array `kernel` (the shape of those dimensions, applied to every leading batch), inverse transform -- one plan, one
+    VkFFTAppend.  The spectral step of a Poisson / Helmholtz solver with Neumann (DCT) or Dirichlet (DST) walls.
+    norm=1: the inverse carries the plan's normalisation, so a kernel of ones returns src; norm=0: unnormalised.
+    Out of place unless dest is src; src is not written then."""
+    import torch
+    if norm not in (0, 1):
+        raise ValueError("norm must be 0 or 1")
+    if kind not in (1, 2, 3, 4):
+        raise ValueError("kind must be 1, 2, 3 or 4")
+    _check(src, "src")
+    if src.is_complex():
+        raise TypeError("real tensor expected")
+    prec = _prec(src, {k: v for k, v in _REAL_PREC.items() if v != 2}, "convolve_r2r")
+    nd, sizes, batch = _split(src.shape, ndim)
+    _check(kernel, "kernel")
+    if kernel.dtype != src.dtype or tuple(kernel.shape) != tuple(src.shape[len(src.shape) - nd:]):
+        raise ValueError(f"kernel must be {tuple(src.shape[len(src.shape) - nd:])} {src.dtype}")
+    inplace = dest is not None and dest.data_ptr() == src.data_ptr()
+    if dest is None:
+        dest = torch.empty_like(src)
+    _check(dest, "dest")
+    if dest.shape != src.shape or dest.dtype != src.dtype:
+        raise ValueError("dest must match src")
+    if kernel.device != src.device or dest.device != src.device:
+        raise ValueError("src, kernel and dest must be on the same device")
+    dev = src.device.index
+    name = "performDST" if dst else "performDCT"
+    fmt = {} if inplace else {"isInputFormatted": 1}
+    app = _plan(("conv_r2r", name, kind, tuple(sizes), batch, prec, norm, dev, inplace), FFTdim=nd, size=sizes,
+                numberBatches=batch, device=dev, doublePrecision=int(prec == 1), normalize=norm, performConvolution=1,
+                **{name: kind}, **fmt)
+    lp = api.VkFFTLaunchParams(buffer=dest, kernel=kernel, stream=_stream(torch, cuda_stream))
+    if not inplace:
+        lp.inputBuffer = src
+    rc = api.VkFFTAppend(app, -1, lp)
+    if rc != 0:
+        raise RuntimeError("VkFFTAppend: " + api.getVkFFTErrorString(rc))
+    return dest
